@@ -2,17 +2,22 @@
 // fp32-grade): the fused per-ray render kernel with the per-sample MLP on Hopper warpgroup MMAs (wgmma,
 // fp32 accumulators in registers).
 //
-// One persistent CTA per SM, NWG + 1 roles:
-//   warpgroups 0..NWG-1  one 64-sample tile each: front end (ray march, NDC, trilinear + colour gather,
-//                        positional encoding -> operand tiles in shared memory), the eight GEMM phases of the
-//                        MLP, their epilogues and the alpha compositing.  Two threads per sample row in the
-//                        front end; in the GEMMs the accumulator fragment of a layer, after bias, modulation and
-//                        ReLU, is converted in registers into the A operand of the next layer (the wgmma
+// One persistent CTA per SM.  fp16-operand modes, warp-specialised (NWG + 2 roles):
+//   warpgroups 0..NWG-1  consumers, one 64-sample tile each: the eight GEMM phases of the MLP, their epilogues
+//                        and the alpha compositing.  The accumulator fragment of a layer, after bias, modulation
+//                        and ReLU, is converted in registers into the A operand of the next layer (the wgmma
 //                        accumulator and register-A layouts coincide), so hidden activations never touch
 //                        shared memory.
-//   warp NWG*4           weight loader: one thread streams the weight image, one K-block of one layer at a
+//   warpgroup NWG        producer: the per-sample front end (ray march, NDC, trilinear + colour gather,
+//                        positional encoding) of the consumers' upcoming tiles, two threads per sample row,
+//                        into a ring of operand-tile slots (PE | MISC, two slots per consumer, full / empty
+//                        mbarriers).  The MMA warpgroups never wait on gathers, and the front end of one tile
+//                        overlaps the GEMMs and epilogues of the others.
+//   last warp            weight loader: one thread streams the weight image, one K-block of one layer at a
 //                        time, L2 -> a shared-memory ring with 1-D bulk async copies (mbarrier complete_tx);
-//                        every warpgroup of the CTA consumes the same chunk sequence.
+//                        every consumer consumes the same chunk sequence.
+// Split mode (hi | lo operands, twice the operand bytes) does not fit the slot ring in shared memory, so there
+// every warpgroup runs its own front end before its GEMMs (NWG + 1 roles, no producer).
 // feature_linear has no non-linearity before views_linears[0] (models.py:213-218): the two are folded at pack
 // time (fp64) into one GEMM from h, with alpha_linear as one extra output row.  Biases are added in fp32 in the
 // epilogues.  Split mode: every operand is x = hi + lo (fp16), three MMAs per K-step (hi*lo + lo*hi + hi*hi),
@@ -27,8 +32,9 @@ namespace mvsn {
 using namespace hop;
 
 namespace wg {
-constexpr int NWG = 2;                                     // tiles in flight per CTA
-constexpr int THREADS = NWG * 128 + 32;
+constexpr int NWG = 2;                                     // MMA warpgroups (tiles in flight) per CTA
+// fp16: NWG consumers + the producer warpgroup + the loader warp; split: NWG warpgroups + the loader warp
+__host__ __device__ constexpr int threads(bool split) { return split ? NWG * 128 + 32 : (NWG + 1) * 128 + 32; }
 constexpr int ROWS = 64;                                   // samples per tile
 constexpr int NCHUNK = 17;
 // B-operand rows of each chunk (one 64-wide K-block of one layer, consumption order):
@@ -42,23 +48,35 @@ constexpr int BIAS_MOD = 0, BIAS_TRUNK = 128, BIAS_HEAD = 896, BIAS_RGB = 968, B
 __host__ __device__ constexpr int tail_offset(bool split) { return NCHUNK * chunk_stride(split); }
 __host__ __device__ constexpr int image_bytes(bool split) { return tail_offset(split) + BIAS_FLOATS * 4; }
 constexpr float SA = 16.f, SW = 256.f;                     // split-mode operand scales
-// shared memory: per warpgroup [PE (hi | lo) | MISC (hi | lo) | modulation fp32 | exchange], then the ring, then the biases
+// shared memory
+//   split: per warpgroup [PE (hi | lo) | MISC (hi | lo) | modulation fp32 | exchange], then the ring, then the biases
+//   fp16:  SLOTS operand-tile slots [PE | MISC], per consumer [modulation fp32 | exchange], then the ring, the biases
+//          = 64 + 2 x 33 + 64 + 4 KB (+ 1 KB alignment) = 199 KB
 __host__ __device__ constexpr int tile_bytes(bool split) { return split ? 16384 : 8192; }
 __host__ __device__ constexpr int off_misc(bool split) { return tile_bytes(split); }
-__host__ __device__ constexpr int off_mod(bool split) { return 2 * tile_bytes(split); }
-__host__ __device__ constexpr int off_xch(bool split) { return off_mod(split) + ROWS * 128 * 4; }
-__host__ __device__ constexpr int wg_bytes(bool split) { return off_xch(split) + 1024; }
+constexpr int MOD_BYTES = ROWS * 128 * 4, XCH_BYTES = 1024;
+constexpr int SLOTS = 2 * NWG;                             // fp16: operand-tile slots, two per consumer
+constexpr int SLOT_BYTES = 2 * 8192;
+__host__ __device__ constexpr int off_mod(bool split) { return 2 * tile_bytes(split); }   // split: inside a warpgroup's region
+__host__ __device__ constexpr int wg_bytes(bool split) { return off_mod(split) + MOD_BYTES + XCH_BYTES; }
+// modulation + exchange of warpgroup w
+__host__ __device__ constexpr int off_state(bool split, int w) {
+    return split ? w * wg_bytes(true) + off_mod(true) : SLOTS * SLOT_BYTES + w * (MOD_BYTES + XCH_BYTES);
+}
 __host__ __device__ constexpr int nstage(bool split) { return split ? 2 : 4; }
-__host__ __device__ constexpr int off_ring(bool split) { return NWG * wg_bytes(split); }
+__host__ __device__ constexpr int off_ring(bool split) { return split ? NWG * wg_bytes(true) : off_state(false, NWG); }
 __host__ __device__ constexpr int off_bias(bool split) { return off_ring(split) + nstage(split) * chunk_stride(split); }
 __host__ __device__ constexpr int smem_bytes(bool split) { return off_bias(split) + BIAS_FLOATS * 4 + 1024; }
 static_assert(smem_bytes(false) <= 227 * 1024 && smem_bytes(true) <= 227 * 1024, "shared memory budget");
-static_assert(wg_bytes(false) % 1024 == 0 && wg_bytes(true) % 1024 == 0, "SW128 tiles need 1024-byte alignment");
+static_assert(wg_bytes(true) % 1024 == 0 && SLOT_BYTES % 1024 == 0 && off_ring(false) % 1024 == 0,
+              "SW128 tiles need 1024-byte alignment");
 }  // namespace wg
 
 struct WgShared {
-    uint64_t full[4];
+    uint64_t full[4];                                      // weight ring
     uint64_t empty[4];
+    uint64_t slot_full[wg::SLOTS];                         // fp16: operand-tile slots
+    uint64_t slot_empty[wg::SLOTS];
     Cams cams;
 };
 
@@ -133,11 +151,151 @@ __device__ __forceinline__ void gemm_rs(float (&d)[N / 2], const uint32_t* ah, c
     }
 }
 
+// ray-march point (px, py, pz), ray direction (dx, dy, dz) and NDC (nx, ny, nz) of sample s_idx of ray `ray`
+template <bool FAST, bool PRECISE>
+__device__ __forceinline__ void sample_point(const SceneDev& sc, const Cams& cams, const RenderIO& io, int ray, int s_idx,
+                                             size_t si, float& px, float& py, float& pz, float& dx, float& dy, float& dz,
+                                             float& nx, float& ny, float& nz) {
+    if (FAST) {
+        const float4* rp = reinterpret_cast<const float4*>(io.rays + (size_t)ray * 8);
+        float4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
+        dx = r0.w; dy = r1.x; dz = r1.y;
+        const float near = r1.z, far = r1.w, tt = __ldg(io.t_steps + s_idx);
+        float zv;
+        if (!io.rg.lindisp) zv = __fadd_rn(__fmul_rn(near, 1.f - tt), __fmul_rn(far, tt));
+        else zv = __fdiv_rn(1.f, __fadd_rn(__fmul_rn(__fdiv_rn(1.f, near), 1.f - tt),
+                                           __fmul_rn(__fdiv_rn(1.f, far), tt)));
+        px = __fadd_rn(r0.x, __fmul_rn(dx, zv));
+        py = __fadd_rn(r0.y, __fmul_rn(dy, zv));
+        pz = __fadd_rn(r0.z, __fmul_rn(dz, zv));
+        ndc_of_point<PRECISE>(sc, cams, io.rg, px, py, pz, nx, ny, nz);
+    } else {
+        px = __ldg(io.pts + si * 3); py = __ldg(io.pts + si * 3 + 1); pz = __ldg(io.pts + si * 3 + 2);
+        nx = __ldg(io.ndc + si * 3); ny = __ldg(io.ndc + si * 3 + 1); nz = __ldg(io.ndc + si * 3 + 2);
+        dx = __ldg(io.dirs + (size_t)ray * 3); dy = __ldg(io.dirs + (size_t)ray * 3 + 1);
+        dz = __ldg(io.dirs + (size_t)ray * 3 + 2);
+    }
+}
+
+// Tile geometry (identical in every role).  A tile is RT rays x SP = 64/RT consecutive samples: row = sub * RT +
+// ray_in, so neighbouring rows are adjacent rays at the SAME sample index -- their volume / image taps fall in the
+// same few cache lines.  Ray and sample of row `row` of tile `tile` of ray group `grp`:
+struct TileRow {
+    int ray, s_idx;
+    bool valid;
+    size_t si;
+    __device__ __forceinline__ TileRow(const RenderIO& io, int grp, int tile, int row) {
+        const int RT = io.rays_per_tile, SP = wg::ROWS / RT, rt_shift = 31 - __clz(RT);
+        ray = grp * RT + (row & (RT - 1));
+        s_idx = tile * SP + (row >> rt_shift);
+        valid = ray < io.N && s_idx < io.S;
+        si = (size_t)ray * io.S + s_idx;
+    }
+};
+
+// Front end of one sample row: the operand columns the consumers' K-steps read.
+//   PE   cols 0..31  = [x y z | sin(2^k x), first 29 of 30]          cols 32..63 = [sin(512 z) | cos(2^k x) | 0]
+//   MISC cols 0..7   = volume features, 8..19 = colour (3 views x (r, g, b, mask)), 20..31 = 0,
+//        cols 32..34 = view direction, 35..47 = 0
+// Two threads per row (part 0 / 1).  fp16 (the producer warpgroup): part 0 takes the volume tap, the view direction
+// and the sines, part 1 the three colour taps and the cosines -- even shares.  Split (each MMA warpgroup runs its own
+// front end): part 0 only the sines, part 1 every gather and the cosines.
+template <bool SPLIT>
+__device__ __forceinline__ void store_pe_sin(uint8_t* pe, int row, const float* nd) {
+    float v[32];
+    v[0] = nd[0]; v[1] = nd[1]; v[2] = nd[2];
+    float f = 1.f;
+#pragma unroll
+    for (int k = 0; k < 10; ++k) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+            if (3 + 3 * k + j < 32) v[3 + 3 * k + j] = SPLIT ? sinf(nd[j] * f) : __sinf(nd[j] * f);
+        f *= 2.f;
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) store8<SPLIT>(pe, row, c, v + 8 * c);
+}
+template <bool SPLIT>
+__device__ __forceinline__ void store_pe_cos(uint8_t* pe, int row, const float* nd) {
+    float v[32];
+    v[0] = SPLIT ? sinf(nd[2] * 512.f) : __sinf(nd[2] * 512.f);
+    float f = 1.f;
+#pragma unroll
+    for (int k = 0; k < 10; ++k) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) v[1 + 3 * k + j] = SPLIT ? cosf(nd[j] * f) : __cosf(nd[j] * f);
+        f *= 2.f;
+    }
+    v[31] = 0.f;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) store8<SPLIT>(pe, row, 4 + c, v + 8 * c);
+}
+// MISC cols 0..7 (volume), 24..31 (zero), 32..39 (view direction), 40..47 (zero); input_feat[0..7]
+template <bool SPLIT>
+__device__ __forceinline__ void store_volume_dir(const SceneDev& sc, const Cams& cams, const RenderIO& io, const TileRow& r,
+                                                 const float* nd, float dx, float dy, float dz, uint8_t* misc, int row) {
+    float feat[8], dir[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) feat[i] = 0.f;
+    if (r.valid) {
+        view_dir<SPLIT>(cams, dx, dy, dz, dir);
+        sample_volume(sc, nd[0], nd[1], nd[2], feat);
+        if (io.input_feat) {
+            float4* o = reinterpret_cast<float4*>(io.input_feat + r.si * 20);
+            o[0] = make_float4(feat[0], feat[1], feat[2], feat[3]);
+            o[1] = make_float4(feat[4], feat[5], feat[6], feat[7]);
+        }
+    }
+    const float z8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    const float d8[8] = {dir[0], dir[1], dir[2], 0.f, 0.f, 0.f, 0.f, 0.f};
+    store8<SPLIT>(misc, row, 0, feat);
+    store8<SPLIT>(misc, row, 3, z8);
+    store8<SPLIT>(misc, row, 4, d8);
+    store8<SPLIT>(misc, row, 5, z8);
+}
+// MISC cols 8..23 (colour, then four zero columns); input_feat[8..19]
+template <bool SPLIT>
+__device__ __forceinline__ void store_color(const SceneDev& sc, const Cams& cams, const RenderIO& io, const TileRow& r,
+                                            float px, float py, float pz, uint8_t* misc, int row) {
+    float feat[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) feat[i] = 0.f;
+    if (r.valid) {
+#pragma unroll
+        for (int vw = 0; vw < 3; ++vw) sample_color<SPLIT>(sc, cams, vw, px, py, pz, feat + 4 * vw);
+        if (io.input_feat) {
+            float4* o = reinterpret_cast<float4*>(io.input_feat + r.si * 20);
+#pragma unroll
+            for (int i = 0; i < 3; ++i) o[2 + i] = make_float4(feat[4 * i], feat[4 * i + 1], feat[4 * i + 2], feat[4 * i + 3]);
+        }
+    }
+    store8<SPLIT>(misc, row, 1, feat);
+    store8<SPLIT>(misc, row, 2, feat + 8);
+}
 template <bool FAST, bool SPLIT>
-__global__ void __launch_bounds__(wg::THREADS, 1)
+__device__ __forceinline__ void front_end(const SceneDev& sc, const Cams& cams, const RenderIO& io, int grp, int tile,
+                                          int t, uint8_t* pe, uint8_t* misc) {
+    const int row = t & (wg::ROWS - 1), part = t >> 6;
+    const TileRow r(io, grp, tile, row);
+    float nx = 0.f, ny = 0.f, nz = 0.f;
+    float px = 0.f, py = 0.f, pz = 0.f, dx = 0.f, dy = 0.f, dz = 1.f;
+    if (r.valid) sample_point<FAST, SPLIT>(sc, cams, io, r.ray, r.s_idx, r.si, px, py, pz, dx, dy, dz, nx, ny, nz);
+    const float nd[3] = {nx, ny, nz};
+    if (part == 0) {
+        if (!SPLIT) store_volume_dir<SPLIT>(sc, cams, io, r, nd, dx, dy, dz, misc, row);
+        store_pe_sin<SPLIT>(pe, row, nd);
+    } else {
+        if (SPLIT) store_volume_dir<SPLIT>(sc, cams, io, r, nd, dx, dy, dz, misc, row);
+        store_color<SPLIT>(sc, cams, io, r, px, py, pz, misc, row);
+        store_pe_cos<SPLIT>(pe, row, nd);
+    }
+}
+
+template <bool FAST, bool SPLIT>
+__global__ void __launch_bounds__(wg::threads(SPLIT), 1)
 render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict__ wimg) {
     using namespace wg;
-    constexpr int NS = nstage(SPLIT);
+    constexpr int NS = nstage(SPLIT), THREADS = threads(SPLIT);
     constexpr float INV = SPLIT ? 1.f / (SA * SW) : 1.f;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -149,26 +307,26 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
     for (int i = tid; i < BIAS_FLOATS; i += THREADS) bias[i] = __ldg(reinterpret_cast<const float*>(wimg + tail_offset(SPLIT)) + i);
     if (tid == 0) {
         for (int i = 0; i < NS; ++i) { mbar_init(&sh.full[i], 1); mbar_init(&sh.empty[i], NWG * 4); }
+        if (!SPLIT)
+            for (int i = 0; i < SLOTS; ++i) { mbar_init(&sh.slot_full[i], 128); mbar_init(&sh.slot_empty[i], 4); }
         fence_barrier_init();
     }
     __syncthreads();
 
     // ---- work decomposition (identical in every role) ---------------------------------------------
-    // A tile is RT rays x SP = 64/RT consecutive samples: row = sub * RT + ray_in, so neighbouring rows are
-    // adjacent rays at the SAME sample index -- their volume / image taps fall in the same few cache lines.
-    // A warpgroup walks the NT tiles of its RT-ray group front to back; the compositing state is carried in
-    // registers.  Any S works.
+    // Warpgroup (consumer) w walks the NT tiles of its RT-ray group front to back; the compositing state is carried
+    // in registers.  Any S works.
     const int N = io.N, S = io.S;
     const int RT = io.rays_per_tile, SP = ROWS / RT;
-    const int rt_shift = 31 - __clz(RT);
     const int NT = (S + SP - 1) / SP;
     const int G = (N + RT - 1) / RT;
     const int units_total = (G + NWG - 1) / NWG;
     const int my_units = blockIdx.x < units_total ? (units_total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
     const int npass = my_units * NT;
     const uint32_t ring = smem_u32(smem + off_ring(SPLIT));
+    auto group_of = [&](int pass, int w) { return ((pass / NT) * (int)gridDim.x + (int)blockIdx.x) * NWG + w; };
 
-    if (warp == NWG * 4) {
+    if (warp == THREADS / 32 - 1) {
         // =========================== weight loader ===================================================
         if (elect_one()) {
             uint32_t n = 0;
@@ -189,17 +347,40 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         }
         return;
     }
+    if constexpr (!SPLIT) {
+        if (warp >= NWG * 4) {
+            // ======================= producer: front ends of the consumers' tiles, in their order ============
+            // consumer w's k-th tile goes to slot 2 w + (k & 1)
+            const int t = tid & 127;
+            uint32_t filled[NWG];
+#pragma unroll
+            for (int w = 0; w < NWG; ++w) filled[w] = 0;
+#pragma unroll 1
+            for (int pass = 0; pass < npass; ++pass) {
+#pragma unroll
+                for (int w = 0; w < NWG; ++w) {
+                    const int grp = group_of(pass, w);
+                    if (grp >= G) continue;
+                    const int s = 2 * w + (filled[w] & 1);
+                    if (filled[w] >= 2) mbar_wait(&sh.slot_empty[s], ((filled[w] >> 1) - 1) & 1);
+                    uint8_t* pe = smem + s * SLOT_BYTES;
+                    front_end<FAST, false>(sc, sh.cams, io, grp, pass % NT, t, pe, pe + tile_bytes(false));
+                    fence_proxy_async();
+                    mbar_arrive(&sh.slot_full[s]);
+                    ++filled[w];
+                }
+            }
+            return;
+        }
+    }
 
-    // =========================== warpgroup: one tile at a time =======================================
+    // =========================== MMA warpgroups: one tile at a time ====================================
     const int wgi = warp >> 2, t = tid & 127, w4 = (tid >> 5) & 3, g = lane >> 2, q = lane & 3;
-    uint8_t* region = smem + wgi * wg_bytes(SPLIT);
-    uint8_t* pe = region;
-    uint8_t* misc = region + off_misc(SPLIT);
-    float* modp = reinterpret_cast<float*>(region + off_mod(SPLIT)) + t;          // [i][128 threads]
-    float* xch = reinterpret_cast<float*>(region + off_xch(SPLIT));                // [64 rows][alpha, r, g, b]
-    const uint32_t pe_u = smem_u32(pe), misc_u = smem_u32(misc);
+    uint8_t* state = smem + off_state(SPLIT, wgi);
+    float* modp = reinterpret_cast<float*>(state) + t;                              // [i][128 threads]
+    float* xch = reinterpret_cast<float*>(state + MOD_BYTES);                       // [64 rows][alpha, r, g, b]
     const int row_a = w4 * 16 + g, row_b = row_a + 8;
-    uint32_t nchunk = 0;
+    uint32_t nchunk = 0, ntile = 0;
     auto acquire = [&]() -> uint32_t {
         const uint32_t st = nchunk % NS;
         mbar_wait(&sh.full[st], (nchunk / NS) & 1);
@@ -218,100 +399,29 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
 
 #pragma unroll 1
     for (int pass = 0; pass < npass; ++pass) {
-        const int grp = ((pass / NT) * (int)gridDim.x + (int)blockIdx.x) * NWG + wgi, tile = pass % NT;
+        const int grp = group_of(pass, wgi), tile = pass % NT;
         if (grp >= G) {                                  // idle in the final passes: keep the weight ring moving
 #pragma unroll 1
             for (int c = 0; c < NCHUNK; ++c) { acquire(); release(); }
             continue;
         }
-        // -------------------------- front end -------------------------------------------------------
-        named_bar_sync(1 + wgi, 128);                    // the previous tile's operand tiles and exchange are consumed
-        {
-            const int row = t & (ROWS - 1), part = t >> 6;
-            const int r_in = row & (RT - 1), s_idx = tile * SP + (row >> rt_shift);
-            const int ray = grp * RT + r_in;
-            const bool valid = ray < N && s_idx < S;
-            const size_t si = (size_t)ray * S + s_idx;
-            float nx = 0.f, ny = 0.f, nz = 0.f;
-            float px = 0.f, py = 0.f, pz = 0.f, dx = 0.f, dy = 0.f, dz = 1.f;
-            if (valid) {
-                if (FAST) {
-                    const float4* rp = reinterpret_cast<const float4*>(io.rays + (size_t)ray * 8);
-                    float4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
-                    dx = r0.w; dy = r1.x; dz = r1.y;
-                    const float near = r1.z, far = r1.w, tt = __ldg(io.t_steps + s_idx);
-                    float zv;
-                    if (!io.rg.lindisp) zv = __fadd_rn(__fmul_rn(near, 1.f - tt), __fmul_rn(far, tt));
-                    else zv = __fdiv_rn(1.f, __fadd_rn(__fmul_rn(__fdiv_rn(1.f, near), 1.f - tt),
-                                                       __fmul_rn(__fdiv_rn(1.f, far), tt)));
-                    px = __fadd_rn(r0.x, __fmul_rn(dx, zv));
-                    py = __fadd_rn(r0.y, __fmul_rn(dy, zv));
-                    pz = __fadd_rn(r0.z, __fmul_rn(dz, zv));
-                    ndc_of_point<SPLIT>(sc, sh.cams, io.rg, px, py, pz, nx, ny, nz);
-                } else {
-                    px = __ldg(io.pts + si * 3); py = __ldg(io.pts + si * 3 + 1); pz = __ldg(io.pts + si * 3 + 2);
-                    nx = __ldg(io.ndc + si * 3); ny = __ldg(io.ndc + si * 3 + 1); nz = __ldg(io.ndc + si * 3 + 2);
-                    dx = __ldg(io.dirs + (size_t)ray * 3); dy = __ldg(io.dirs + (size_t)ray * 3 + 1);
-                    dz = __ldg(io.dirs + (size_t)ray * 3 + 2);
-                }
-            }
-            const float nd[3] = {nx, ny, nz};
-            if (part == 0) {
-                // PE cols 0..31 = [x y z | sin(2^k x), first 29 of 30]
-                float v[32];
-                v[0] = nx; v[1] = ny; v[2] = nz;
-                float f = 1.f;
-#pragma unroll
-                for (int k = 0; k < 10; ++k) {
-#pragma unroll
-                    for (int j = 0; j < 3; ++j)
-                        if (3 + 3 * k + j < 32) v[3 + 3 * k + j] = SPLIT ? sinf(nd[j] * f) : __sinf(nd[j] * f);
-                    f *= 2.f;
-                }
-#pragma unroll
-                for (int c = 0; c < 4; ++c) store8<SPLIT>(pe, row, c, v + 8 * c);
-            } else {
-                // all gathers: volume (8) + colour (12) features -> MISC cols 0..19, view direction -> cols 32..34;
-                // PE cols 32..63 = [sin(512 z) | cos | 0]
-                float feat[24], dir[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-                for (int i = 0; i < 24; ++i) feat[i] = 0.f;
-                if (valid) {
-                    view_dir<SPLIT>(sh.cams, dx, dy, dz, dir);
-                    sample_volume(sc, nx, ny, nz, feat);
-#pragma unroll
-                    for (int v = 0; v < 3; ++v) sample_color<SPLIT>(sc, sh.cams, v, px, py, pz, feat + 8 + 4 * v);
-                    if (io.input_feat) {
-                        float4* o = reinterpret_cast<float4*>(io.input_feat + si * 20);
-#pragma unroll
-                        for (int i = 0; i < 5; ++i)
-                            o[i] = make_float4(feat[4 * i], feat[4 * i + 1], feat[4 * i + 2], feat[4 * i + 3]);
-                    }
-                }
-                store8<SPLIT>(misc, row, 0, feat);
-                store8<SPLIT>(misc, row, 1, feat + 8);
-                store8<SPLIT>(misc, row, 2, feat + 16);
-                const float z8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                store8<SPLIT>(misc, row, 3, z8);
-                const float d8[8] = {dir[0], dir[1], dir[2], 0.f, 0.f, 0.f, 0.f, 0.f};
-                store8<SPLIT>(misc, row, 4, d8);
-                store8<SPLIT>(misc, row, 5, z8);
-                float v[32];
-                v[0] = SPLIT ? sinf(nz * 512.f) : __sinf(nz * 512.f);
-                float f = 1.f;
-#pragma unroll
-                for (int k = 0; k < 10; ++k) {
-#pragma unroll
-                    for (int j = 0; j < 3; ++j) v[1 + 3 * k + j] = SPLIT ? cosf(nd[j] * f) : __cosf(nd[j] * f);
-                    f *= 2.f;
-                }
-                v[31] = 0.f;
-#pragma unroll
-                for (int c = 0; c < 4; ++c) store8<SPLIT>(pe, row, 4 + c, v + 8 * c);
-            }
+        uint32_t pe_u, misc_u, slot = 0;
+        named_bar_sync(1 + wgi, 128);                    // the previous tile's exchange (split: operand tiles) is consumed
+        if constexpr (SPLIT) {
+            // -------------------------- front end (split mode: this warpgroup's own operand tiles) -------------
+            uint8_t* pe = smem + wgi * wg_bytes(true);
+            uint8_t* misc = pe + off_misc(true);
+            front_end<FAST, true>(sc, sh.cams, io, grp, tile, t, pe, misc);
+            fence_proxy_async();
+            named_bar_sync(1 + wgi, 128);
+            pe_u = smem_u32(pe); misc_u = smem_u32(misc);
+        } else {
+            // -------------------------- operand tiles from the producer -----------------------------------
+            slot = 2 * wgi + (ntile & 1);
+            mbar_wait(&sh.slot_full[slot], (ntile >> 1) & 1);
+            ++ntile;
+            pe_u = smem_u32(smem + slot * SLOT_BYTES); misc_u = pe_u + tile_bytes(false);
         }
-        fence_proxy_async();
-        named_bar_sync(1 + wgi, 128);
 
         // -------------------------- modulation: pts_bias(features), K = 20 -> kept in shared memory ---------
         {
@@ -388,6 +498,9 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                 gemm_ss<72, SPLIT>(h72, misc_u, b, 2, 1, false);
                 wgmma_commit(); wgmma_wait<0>(); reg_fence(h72);
                 release();
+                if constexpr (!SPLIT) {                // the last read of the operand tiles: free the slot
+                    if (lane == 0) mbar_arrive(&sh.slot_empty[slot]);
+                }
             }
 #pragma unroll
             for (int i = 0; i < 32; i += 2) {
@@ -481,13 +594,13 @@ int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool 
     const int grid = units < sm_count() ? units : sm_count();
     if (grid <= 0) return MVSN_OK;
     const uint8_t* w = static_cast<const uint8_t*>(wimg);
-    const int smem = smem_bytes(split);
+    const int smem = smem_bytes(split), nthreads = threads(split);
     if (split) {
-        if (fast) render_wg_kernel<true, true><<<grid, THREADS, smem, stream>>>(sc, io, w);
-        else      render_wg_kernel<false, true><<<grid, THREADS, smem, stream>>>(sc, io, w);
+        if (fast) render_wg_kernel<true, true><<<grid, nthreads, smem, stream>>>(sc, io, w);
+        else      render_wg_kernel<false, true><<<grid, nthreads, smem, stream>>>(sc, io, w);
     } else {
-        if (fast) render_wg_kernel<true, false><<<grid, THREADS, smem, stream>>>(sc, io, w);
-        else      render_wg_kernel<false, false><<<grid, THREADS, smem, stream>>>(sc, io, w);
+        if (fast) render_wg_kernel<true, false><<<grid, nthreads, smem, stream>>>(sc, io, w);
+        else      render_wg_kernel<false, false><<<grid, nthreads, smem, stream>>>(sc, io, w);
     }
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;
