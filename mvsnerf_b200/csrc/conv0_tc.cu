@@ -11,8 +11,9 @@
 // whole resident weight matrix (224 x 48), and the "im2col" never exists.
 //
 // fp32-grade accuracy (the volume gate is 1e-4 |v|max): 2-term fp16 operand split, three MMAs per K-step
-// (hi*hi + hi*lo + lo*hi into one fp32 accumulator), operands carried with exact power-of-two scales (x16 inputs,
-// x256 weights) so that the lo terms stay normal fp16 numbers -- the scheme of render_wg.cu's split mode.
+// (hi*hi + hi*lo + lo*hi into one fp32 accumulator), weights carried x256 (an exact power of two) so that their lo
+// terms stay normal fp16 numbers.  The inputs are split unscaled: any |cost| < 65504 stays finite (a x16 scale would
+// overflow fp16 at |cost| = 4095).
 //
 // One persistent CTA per SM walks bricks of 6 x 10 x 24 output voxels (halo brick 8 x 12 x 32 positions = 24 operand
 // tiles of 128 positions; a tile = 4 x-rows of 32 positions):
@@ -45,7 +46,7 @@ constexpr int HZ = BZ + 2, HY = BY + 2, HX = 32;        // halo brick (x: one wa
 static_assert(BX % 4 == 0 && XOFF % 4 == 0 && XOFF >= 1 && XOFF + BX + 1 <= HX, "x window");
 constexpr int TILES = HZ * HY * HX / 128;               // 24 operand tiles per brick
 constexpr int NCOL = 224;                               // 27 taps x 8 channels = 216, padded to a multiple of 16
-constexpr float SA = 16.f, SW = 256.f, INV_SCALE = 1.f / (16.f * 256.f);
+constexpr float SW = 256.f, INV_SCALE = 1.f / 256.f;
 constexpr int W_PART = NCOL * 128;                      // bytes of the hi (or lo) weight image: [224][64] fp16, SW128
 constexpr int A_PART = 128 * 128;                       // bytes of the hi (or lo) operand tile
 constexpr int OFF_W = 0;                                // hi | lo
@@ -262,7 +263,7 @@ conv0_tc_kernel(const ConvArgs a, const __grid_constant__ CUtensorMap tmap, cons
                 for (int half = 0; half < 2; ++half) {
                     uint32_t h[4], l[4];
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) split2_c0(v[half * 8 + 2 * j] * SA, v[half * 8 + 2 * j + 1] * SA, h[j], l[j]);
+                    for (int j = 0; j < 4; ++j) split2_c0(v[half * 8 + 2 * j], v[half * 8 + 2 * j + 1], h[j], l[j]);
                     const uint32_t off = sw128_offset(row, (k2 * 2 + half) * 8);
                     *reinterpret_cast<uint4*>(hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
                     *reinterpret_cast<uint4*>(hi + A_PART + off) = make_uint4(l[0], l[1], l[2], l[3]);

@@ -21,7 +21,15 @@
 // feature_linear has no non-linearity before views_linears[0] (models.py:213-218): the two are folded at pack
 // time (fp64) into one GEMM from h, with alpha_linear as one extra output row.  Biases are added in fp32 in the
 // epilogues.  Split mode: every operand is x = hi + lo (fp16), three MMAs per K-step (hi*lo + lo*hi + hi*hi),
-// activations carried x16 and weights x256 (exact powers of two, undone in the epilogue).
+// with exact power-of-two scales, undone in the epilogues:
+//   front-end operands (encoding, features, view direction)  none: |x| < 65504
+//   weights                                                   2^ew for the whole image: x256, lowered when the largest
+//                                                             |w| reaches 128 so that it packs below 2^15
+//   hidden activations                                        2^e per sample row, chosen by the epilogue that makes the
+//                                                             row: its maximum lands in [2^14, 2^15), whatever the range
+// The four threads of a quad hold a whole accumulator row, so the row maximum costs two shuffles, and the same thread
+// holds that row in the next GEMM's accumulator.  Where one GEMM reads front-end columns and register columns (layer 5,
+// folded head), the fp32 accumulator rows are rescaled exactly between the two groups of K-blocks.
 //
 // Replaces renderer.rendering (renderer.py:138-165) and callees; see include/mvsnerf_b200.h.
 #include "render_frontend.cuh"
@@ -43,11 +51,11 @@ constexpr int NCHUNK = 17;
 __host__ __device__ constexpr int chunk_rows(int c) { return c >= 13 && c <= 15 ? 72 : c == 16 ? 8 : 128; }
 constexpr int HALF_STRIDE = 16384;                         // bytes of one fp16 image of a chunk (hi; lo follows in split mode)
 __host__ __device__ constexpr int chunk_stride(bool split) { return split ? 2 * HALF_STRIDE : HALF_STRIDE; }
-// fp32 bias tail after the chunks
-constexpr int BIAS_MOD = 0, BIAS_TRUNK = 128, BIAS_HEAD = 896, BIAS_RGB = 968, BIAS_FLOATS = 1024;
+// fp32 bias tail after the chunks; split mode also keeps there the largest |weight| (fp32 bits) and 2^-ew
+constexpr int BIAS_MOD = 0, BIAS_TRUNK = 128, BIAS_HEAD = 896, BIAS_RGB = 968, BIAS_WINV = 1016, BIAS_WMAX = 1017,
+              BIAS_FLOATS = 1024;
 __host__ __device__ constexpr int tail_offset(bool split) { return NCHUNK * chunk_stride(split); }
 __host__ __device__ constexpr int image_bytes(bool split) { return tail_offset(split) + BIAS_FLOATS * 4; }
-constexpr float SA = 16.f, SW = 256.f;                     // split-mode operand scales
 // shared memory
 //   split: per warpgroup [PE (hi | lo) | MISC (hi | lo) | modulation fp32 | exchange], then the ring, then the biases
 //   fp16:  SLOTS operand-tile slots [PE | MISC], per consumer [modulation fp32 | exchange], then the ring, the biases
@@ -98,6 +106,41 @@ __device__ __forceinline__ void split_h2(float a, float b, uint32_t& hi, uint32_
     hi = *reinterpret_cast<const uint32_t*>(&h);
     lo = *reinterpret_cast<const uint32_t*>(&l);
 }
+// split mode: 2^(14 - floor(log2 m)) for a row maximum m >= 0 (clamped to [2^-113, 2^54]; a zero row takes any scale)
+__device__ __forceinline__ float row_scale(float m) {
+    const int eb = min(max((__float_as_int(m) >> 23) & 0xff, 87), 254);
+    return __int_as_float((268 - eb) << 23);
+}
+__device__ __forceinline__ float inv_pow2(float s) { return __int_as_float((254 << 23) - __float_as_int(s)); }
+// split mode: hidden activations v (>= 0, accumulator layout: v[i] is row row_a if (i & 2) == 0, else row_b) ->
+// hi / lo A registers of the next GEMM, each row scaled by sa / sb so that its maximum lies in [2^14, 2^15)
+template <int NV>
+__device__ __forceinline__ void split_rows(const float* v, uint32_t* ah, uint32_t* al, float& sa, float& sb) {
+    float pa[4] = {0.f, 0.f, 0.f, 0.f}, pb[4] = {0.f, 0.f, 0.f, 0.f};   // four short chains per row, not one long one
+#pragma unroll
+    for (int j = 0; j < NV / 4; ++j) {
+        pa[j & 3] = fmaxf(pa[j & 3], fmaxf(v[4 * j], v[4 * j + 1]));
+        pb[j & 3] = fmaxf(pb[j & 3], fmaxf(v[4 * j + 2], v[4 * j + 3]));
+    }
+    float ma = fmaxf(fmaxf(pa[0], pa[1]), fmaxf(pa[2], pa[3])), mb = fmaxf(fmaxf(pb[0], pb[1]), fmaxf(pb[2], pb[3]));
+    ma = fmaxf(ma, __shfl_xor_sync(0xffffffffu, ma, 1)); ma = fmaxf(ma, __shfl_xor_sync(0xffffffffu, ma, 2));
+    mb = fmaxf(mb, __shfl_xor_sync(0xffffffffu, mb, 1)); mb = fmaxf(mb, __shfl_xor_sync(0xffffffffu, mb, 2));
+    sa = row_scale(ma); sb = row_scale(mb);
+#pragma unroll
+    for (int i = 0; i < NV; i += 2) {
+        const float s = (i & 2) ? sb : sa;
+        split_h2(v[i] * s, v[i + 1] * s, ah[i >> 1], al[i >> 1]);
+    }
+}
+// split mode: the weight scale 2^ew from the largest |weight| (fp32 bits): 256 unless that would put it above 2^15
+__host__ __device__ inline float weight_scale(uint32_t wmax_bits) {
+    int eb = (int)(wmax_bits >> 23) & 0xff;
+    eb = eb < 1 ? 1 : eb > 254 ? 254 : eb;
+    const int e = 141 - eb < 8 ? 141 - eb : 8;               // 14 - floor(log2 |w|max), at most 8
+    union { uint32_t u; float f; } r;
+    r.u = (uint32_t)(e + 127) << 23;
+    return r.f;
+}
 
 // eight consecutive operand columns (16-byte chunk c) of `row` into a SW128 tile; split: lo image 8 KB after hi
 template <bool SPLIT>
@@ -106,7 +149,7 @@ __device__ __forceinline__ void store8(uint8_t* tile, int row, int c, const floa
     if (SPLIT) {
         uint32_t h[4], l[4];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) split_h2(v[2 * j] * wg::SA, v[2 * j + 1] * wg::SA, h[j], l[j]);
+        for (int j = 0; j < 4; ++j) split_h2(v[2 * j], v[2 * j + 1], h[j], l[j]);
         *reinterpret_cast<uint4*>(tile + off) = make_uint4(h[0], h[1], h[2], h[3]);
         *reinterpret_cast<uint4*>(tile + 8192 + off) = make_uint4(l[0], l[1], l[2], l[3]);
     } else {
@@ -296,7 +339,6 @@ __global__ void __launch_bounds__(wg::threads(SPLIT), 1)
 render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict__ wimg) {
     using namespace wg;
     constexpr int NS = nstage(SPLIT), THREADS = threads(SPLIT);
-    constexpr float INV = SPLIT ? 1.f / (SA * SW) : 1.f;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     __shared__ WgShared sh;
@@ -396,6 +438,10 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
     float cT = 1.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f, c4 = 0.f;   // compositing state of ray t (t < RT)
     float acc[64];
     uint32_t ah[32], al[SPLIT ? 32 : 1];
+    // split: 2^-ew, the scale of the register activation rows row_a / row_b, and the factor that takes the current
+    // accumulator rows back to their true values (fp16: all 1)
+    const float inv_w = SPLIT ? bias[BIAS_WINV] : 1.f;
+    float sa = 1.f, sb = 1.f, ia = inv_w, ib = inv_w;
 
 #pragma unroll 1
     for (int pass = 0; pass < npass; ++pass) {
@@ -431,17 +477,24 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             wgmma_commit(); wgmma_wait<0>(); reg_fence(acc);
             release();
 #pragma unroll
-            for (int i = 0; i < 64; ++i) modp[i * 128] = fmaf(acc[i], INV, bias[BIAS_MOD + col_of(i)]);
+            for (int i = 0; i < 64; ++i) modp[i * 128] = fmaf(acc[i], inv_w, bias[BIAS_MOD + col_of(i)]);
         }
         // -------------------------- trunk: six layers, h = relu((W x + b) * mod) -----------------------------
         auto trunk_epilogue = [&](int l) {
+            if constexpr (SPLIT) {
 #pragma unroll
-            for (int i = 0; i < 64; i += 2) {
-                float v0 = fmaf(acc[i], INV, bias[BIAS_TRUNK + l * 128 + col_of(i)]) * modp[i * 128];
-                float v1 = fmaf(acc[i + 1], INV, bias[BIAS_TRUNK + l * 128 + col_of(i + 1)]) * modp[(i + 1) * 128];
-                v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
-                if (SPLIT) split_h2(v0 * SA, v1 * SA, ah[i >> 1], al[(i >> 1) & (SPLIT ? 31 : 0)]);
-                else ah[i >> 1] = cvt_h2_sat(v0, v1);
+                for (int i = 0; i < 64; ++i)
+                    acc[i] = fmaxf(fmaf(acc[i], (i & 2) ? ib : ia, bias[BIAS_TRUNK + l * 128 + col_of(i)]) * modp[i * 128], 0.f);
+                split_rows<64>(acc, ah, al, sa, sb);
+                ia = inv_pow2(sa) * inv_w; ib = inv_pow2(sb) * inv_w;
+            } else {
+#pragma unroll
+                for (int i = 0; i < 64; i += 2) {
+                    float v0 = (acc[i] + bias[BIAS_TRUNK + l * 128 + col_of(i)]) * modp[i * 128];
+                    float v1 = (acc[i + 1] + bias[BIAS_TRUNK + l * 128 + col_of(i + 1)]) * modp[(i + 1) * 128];
+                    v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
+                    ah[i >> 1] = cvt_h2_sat(v0, v1);
+                }
             }
         };
         {   // layer 0: A = encoding (63 columns)
@@ -450,6 +503,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             gemm_ss<128, SPLIT>(acc, pe_u, b, 0, 4, true);
             wgmma_commit(); wgmma_wait<0>(); reg_fence(acc);
             release();
+            ia = ib = inv_w;
             trunk_epilogue(0);
         }
 #pragma unroll 1
@@ -470,6 +524,10 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             gemm_ss<128, SPLIT>(acc, pe_u, b, 0, 4, true);
             wgmma_commit(); wgmma_wait<0>(); reg_fence(acc);
             release();
+            if constexpr (SPLIT) {                     // to the scale of the register rows (exact: powers of two)
+#pragma unroll
+                for (int i = 0; i < 64; ++i) acc[i] *= (i & 2) ? sb : sa;
+            }
 #pragma unroll
             for (int kb = 0; kb < 2; ++kb) {
                 b = acquire();
@@ -492,6 +550,11 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                 wgmma_commit(); wgmma_wait<0>(); reg_fence(h72);
                 release();
             }
+            if constexpr (SPLIT) {                     // back to the front-end scale of the view-direction columns
+                const float ra = inv_pow2(sa), rb = inv_pow2(sb);
+#pragma unroll
+                for (int i = 0; i < 36; ++i) h72[i] *= (i & 2) ? rb : ra;
+            }
             {   // view direction: MISC K-step 2 (cols 32..47)
                 const uint32_t b = acquire();
                 wgmma_fence();
@@ -502,15 +565,21 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                     if (lane == 0) mbar_arrive(&sh.slot_empty[slot]);
                 }
             }
+            if constexpr (SPLIT) {
 #pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-                const float v0 = fmaxf(fmaf(h72[i], INV, bias[BIAS_HEAD + col_of(i)]), 0.f);
-                const float v1 = fmaxf(fmaf(h72[i + 1], INV, bias[BIAS_HEAD + col_of(i + 1)]), 0.f);
-                if (SPLIT) split_h2(v0 * SA, v1 * SA, ah[i >> 1], al[(i >> 1) & (SPLIT ? 31 : 0)]);
-                else ah[i >> 1] = cvt_h2_sat(v0, v1);
+                for (int i = 0; i < 32; ++i) h72[i] = fmaxf(fmaf(h72[i], inv_w, bias[BIAS_HEAD + col_of(i)]), 0.f);
+                split_rows<32>(h72, ah, al, sa, sb);
+                ia = inv_pow2(sa) * inv_w; ib = inv_pow2(sb) * inv_w;
+            } else {
+#pragma unroll
+                for (int i = 0; i < 32; i += 2) {
+                    const float v0 = fmaxf(h72[i] + bias[BIAS_HEAD + col_of(i)], 0.f);
+                    const float v1 = fmaxf(h72[i + 1] + bias[BIAS_HEAD + col_of(i + 1)], 0.f);
+                    ah[i >> 1] = cvt_h2_sat(v0, v1);
+                }
             }
-            sig_a = fmaxf(fmaf(h72[32], INV, bias[BIAS_HEAD + 64]), 0.f);
-            sig_b = fmaxf(fmaf(h72[34], INV, bias[BIAS_HEAD + 64]), 0.f);
+            sig_a = fmaxf(fmaf(h72[32], inv_w, bias[BIAS_HEAD + 64]), 0.f);
+            sig_b = fmaxf(fmaf(h72[34], inv_w, bias[BIAS_HEAD + 64]), 0.f);
         }
         // -------------------------- rgb (N = 8, 3 used) -------------------------------------------------------
         {
@@ -524,13 +593,13 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             if (q == 0) {
                 xch[row_a * 4 + 0] = 1.f - (SPLIT ? expf(-sig_a) : __expf(-sig_a));
                 xch[row_b * 4 + 0] = 1.f - (SPLIT ? expf(-sig_b) : __expf(-sig_b));
-                xch[row_a * 4 + 1] = sigm(fmaf(r8[0], INV, bias[BIAS_RGB + 0]));
-                xch[row_a * 4 + 2] = sigm(fmaf(r8[1], INV, bias[BIAS_RGB + 1]));
-                xch[row_b * 4 + 1] = sigm(fmaf(r8[2], INV, bias[BIAS_RGB + 0]));
-                xch[row_b * 4 + 2] = sigm(fmaf(r8[3], INV, bias[BIAS_RGB + 1]));
+                xch[row_a * 4 + 1] = sigm(fmaf(r8[0], ia, bias[BIAS_RGB + 0]));
+                xch[row_a * 4 + 2] = sigm(fmaf(r8[1], ia, bias[BIAS_RGB + 1]));
+                xch[row_b * 4 + 1] = sigm(fmaf(r8[2], ib, bias[BIAS_RGB + 0]));
+                xch[row_b * 4 + 2] = sigm(fmaf(r8[3], ib, bias[BIAS_RGB + 1]));
             } else if (q == 1) {
-                xch[row_a * 4 + 3] = sigm(fmaf(r8[0], INV, bias[BIAS_RGB + 2]));
-                xch[row_b * 4 + 3] = sigm(fmaf(r8[2], INV, bias[BIAS_RGB + 2]));
+                xch[row_a * 4 + 3] = sigm(fmaf(r8[0], ia, bias[BIAS_RGB + 2]));
+                xch[row_b * 4 + 3] = sigm(fmaf(r8[2], ib, bias[BIAS_RGB + 2]));
             }
         }
         named_bar_sync(1 + wgi, 128);
@@ -607,7 +676,7 @@ int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool 
 }
 
 // ------------------------------------------------------------------------------------------------
-// weight image packer (fp32 nn.Linear tensors -> fp16 (split: hi | lo, x256) pre-swizzled chunks + fp32 biases)
+// weight image packer (fp32 nn.Linear tensors -> fp16 (split: hi | lo, x2^ew) pre-swizzled chunks + fp32 biases)
 // ------------------------------------------------------------------------------------------------
 struct MlpPtrsWg { const float* p[MVSN_N_MLP_TENSORS]; };
 
@@ -631,12 +700,24 @@ __device__ float wg_weight(const MlpPtrsWg& w, int c, int r, int k) {
     return r < 3 ? w.p[20][r * 64 + k] : 0.f;
 }
 
+// split mode: the largest |weight| of the image (its fp32 bits; atomicMax orders non-negative floats) -> tail[BIAS_WMAX],
+// which the caller has zeroed
+__global__ void wmax_mlp_wg_kernel(MlpPtrsWg w, uint8_t* __restrict__ out) {
+    using namespace wg;
+    const int c = blockIdx.x;
+    float m = 0.f;
+    for (int i = threadIdx.x; i < chunk_rows(c) * 64; i += blockDim.x) m = fmaxf(m, fabsf(wg_weight(w, c, i >> 6, i & 63)));
+    atomicMax(reinterpret_cast<unsigned int*>(out + tail_offset(true)) + BIAS_WMAX, __float_as_uint(m));
+}
+
 __global__ void pack_mlp_wg_kernel(MlpPtrsWg w, bool split, uint8_t* __restrict__ out) {
     using namespace wg;
     const int c = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+    const float sw = split ? weight_scale(reinterpret_cast<const uint32_t*>(out + tail_offset(true))[BIAS_WMAX]) : 1.f;
     if (c == NCHUNK) {                             // fp32 bias tail
         float* b = reinterpret_cast<float*>(out + tail_offset(split));
         for (int i = tid; i < BIAS_FLOATS; i += nt) {
+            if (split && i == BIAS_WMAX) continue;
             float v = 0.f;
             if (i < BIAS_TRUNK) v = w.p[13][i];
             else if (i < BIAS_HEAD) { const int l = (i - BIAS_TRUNK) / 128; v = w.p[2 * l + 1][(i - BIAS_TRUNK) % 128]; }
@@ -647,6 +728,7 @@ __global__ void pack_mlp_wg_kernel(MlpPtrsWg w, bool split, uint8_t* __restrict_
                 v = (float)s;
             } else if (i == BIAS_HEAD + 64) v = w.p[19][0];
             else if (i >= BIAS_RGB && i < BIAS_RGB + 3) v = w.p[21][i - BIAS_RGB];
+            else if (split && i == BIAS_WINV) v = 1.f / sw;
             b[i] = v;
         }
         return;
@@ -659,9 +741,9 @@ __global__ void pack_mlp_wg_kernel(MlpPtrsWg w, bool split, uint8_t* __restrict_
         const uint32_t off = sw128_offset(r, k);
         const float v = wg_weight(w, c, r, k);
         if (split) {
-            const __half h = __float2half_rn(v * SW);
+            const __half h = __float2half_rn(v * sw);
             *reinterpret_cast<__half*>(dst + off) = h;
-            *reinterpret_cast<__half*>(dst + HALF_STRIDE + off) = __float2half_rn(v * SW - __half2float(h));
+            *reinterpret_cast<__half*>(dst + HALF_STRIDE + off) = __float2half_rn(v * sw - __half2float(h));
         } else {
             *reinterpret_cast<__half*>(dst + off) = __float2half_rn(v);
         }
@@ -673,6 +755,12 @@ size_t mlp_wg_packed_bytes(bool split) { return wg::image_bytes(split); }
 int pack_mlp_wg(const float* const* w, bool split, void* packed, cudaStream_t stream) {
     MlpPtrsWg p;
     for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) p.p[i] = w[i];
+    if (split) {
+        uint8_t* wmax = static_cast<uint8_t*>(packed) + wg::tail_offset(true) + wg::BIAS_WMAX * 4;
+        MVSN_CUDA_CHECK(cudaMemsetAsync(wmax, 0, 4, stream));
+        wmax_mlp_wg_kernel<<<wg::NCHUNK, 256, 0, stream>>>(p, static_cast<uint8_t*>(packed));
+        MVSN_CUDA_CHECK(cudaGetLastError());
+    }
     pack_mlp_wg_kernel<<<wg::NCHUNK + 1, 256, 0, stream>>>(p, split, static_cast<uint8_t*>(packed));
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;
