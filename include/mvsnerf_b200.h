@@ -279,10 +279,6 @@ int mvsn_costreg_forward_bn(const float* const* w_host_array_of_device_ptrs, flo
  * the fused render kernel uses.  A [128,K], B [N,K] fp16 row-major; Bc [N,16] optional extra K-step
  * (D += A[:,16:32] * Bc^T, the "bias" step); D [128,N] fp32.  Used by tests only.
  * ------------------------------------------------------------------------------------- */
-/* Debug: when non-NULL, CTA 0 of the tensor-core render kernel records a clock64 timeline of its
- * pipeline events into this device buffer (8 roles x 1024 entries).  NULL (default) disables it. */
-void mvsn_debug_set_trace(long long* device_buffer);
-
 int mvsn_selftest_umma(const void* A, const void* B, const void* Bc, int N, int K, float* D, void* stream);
 
 #ifdef __cplusplus

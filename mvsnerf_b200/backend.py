@@ -545,13 +545,14 @@ def _render_samples_torch(pts, ndc, z, rays_dir, vol, imgs, w2cs, intrinsics, ne
 
 
 class _RenderSamplesFn(torch.autograd.Function):
-    """Training-step form of `rendering` (SURVEY.md 8(f) row 2, interim).
+    """Training-step form of `rendering` (SURVEY.md 8(f) row 2).
 
     forward: the fused CUDA kernel, exactly as in inference (no graph, nothing per-sample kept).
-    backward: gradients w.r.t. the 22 MLP tensors and the encoding volume by re-evaluating the chunk with
-    PyTorch ops under autograd (_render_samples_torch) -- activation memory exists only during backward.
-    A hand-written backward kernel (MLP dgrad/wgrad + trilinear scatter) is the planned replacement; the
-    interface (what is differentiable, what re-packs after an optimiser step) will not change."""
+    backward: gradients w.r.t. the 22 MLP tensors and the encoding volume.  With N_samples <= 128 (and
+    BACKWARD_IMPL == "kernel") they come from the backward kernel (csrc/render_bwd.cu: forward recompute on the
+    fp32 render kernel's own forward tile, MLP dgrad/wgrad, trilinear scatter into the volume gradient).  Otherwise
+    the chunk is re-evaluated with PyTorch ops under autograd (_render_samples_torch); activation memory then
+    exists only during backward."""
 
     @staticmethod
     def forward(ctx, pts, ndc, z, rays_dir, vol, imgs, w2cs, intrinsics, white_bkgd, mode, network_fn, volume_feature,

@@ -119,8 +119,6 @@ __global__ void pack_mlp_fp32_kernel(MlpPtrs w, float* __restrict__ out) {
     copy_into(out + BR, w.p[I_BR], 3, 4, tid, nt);
 }
 
-static long long* g_trace = nullptr;
-
 static int make_scene(const mvsn_render_scene* s, SceneDev& d) {
     MVSN_REQUIRE(s != nullptr, MVSN_ENULL, "scene is NULL");
     MVSN_REQUIRE(s->volume_dhwc && s->imgs_hwc4 && s->mlp_packed, MVSN_ENULL, "scene has a NULL buffer");
@@ -159,8 +157,7 @@ using namespace mvsn;
 extern "C" {
 
 const char* mvsn_last_error(void) { return g_err; }
-int mvsn_abi_version(void) { return 1; }
-void mvsn_debug_set_trace(long long* device_buffer) { g_trace = device_buffer; }
+int mvsn_abi_version(void) { return 2; }
 
 size_t mvsn_mlp_packed_bytes(int mode) {
     switch (mode) {
@@ -240,7 +237,6 @@ int mvsn_render_samples(const mvsn_render_scene* scene, const float* rays_pts, c
     io.pts = rays_pts; io.ndc = rays_ndc; io.z = z_vals; io.dirs = rays_dir;
     io.N = N; io.S = S;
     io.rgb = rgb; io.depth = depth; io.weights = weights; io.alpha = alpha; io.input_feat = input_feat;
-    io.trace = g_trace;
     return dispatch_render(scene, sc, io, false, (cudaStream_t)stream);
 }
 
@@ -270,7 +266,6 @@ static int render_rays_impl(const mvsn_render_scene* scene, const mvsn_ray_param
     io.rg.wf = (float)scene->W / 4.0f;     // (inv_scale + 1) / 4, utils.py:139
     io.rg.hf = (float)scene->H / 4.0f;
     io.rg.lindisp = rp->lindisp;
-    io.trace = g_trace;
     if (sink) {
         MVSN_REQUIRE(sink->n_peers >= 1 && sink->n_peers <= MVSN_MAX_PEERS, MVSN_EBADSHAPE,
                      "peer sink: n_peers=%d (1..%d)", sink->n_peers, MVSN_MAX_PEERS);

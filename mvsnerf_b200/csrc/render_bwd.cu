@@ -4,15 +4,16 @@
 // 22 MLP tensors (models.py:145-222) and RefVolume.feat_volume (models.py:935-950).  What autograd computes there
 // with ~200 library launches per step is done here by
 //
-//   render_bwd_kernel      per tile of 128 samples: recompute the forward (fp32 FFMA, same passes as render_fp32.cu),
+//   render_bwd_kernel      per tile of 128 samples: recompute the forward with the fp32 render kernel's own forward
+//                          tile (tile_fp32.cuh; N_samples <= 128, so a tile holds whole rays and needs no chunk carry),
 //                          reverse compositing scan, MLP dgrad + wgrad as tiled GEMMs, trilinear scatter-add of the
 //                          8 volume-feature gradients into the channels-last volume gradient;
 //   mlp_grad_reduce_kernel per-CTA private weight-gradient accumulators -> the 22 tensors in nn.Linear layout;
 //   adam_*_kernel          fused Adam (torch.optim.Adam arithmetic) on the MLP tensors and on the volume.
 //
 // Data flow of a tile (one persistent CTA of 256 threads per SM, 7 tiles per CTA at 1024 rays x 128 samples):
-//   * forward recompute keeps what the backward needs in a per-CTA scratch in global memory (704 KB, L2 resident):
-//     the layer outputs TRANSPOSED (hT[n][r]) -- that is exactly the A operand of the wgrad GEMM
+//   * the forward recompute records (ScratchRecord) what the backward needs in a per-CTA scratch in global memory
+//     (704 KB, L2 resident): the layer outputs TRANSPOSED (hT[n][r]) -- that is exactly the A operand of the wgrad GEMM
 //     dW^T[k][n] = sum_r x^T[k][r] dpre[r][n], and the element-wise stage reads the same fragment shape from it;
 //   * the pre-activation is not stored: h = relu(pre * mod) > 0  =>  pre = h / mod, and the sample does not
 //     contribute where h == 0;
@@ -23,8 +24,7 @@
 //     the only atomics are the volume scatter (red.global.add.v4.f32, 16 per sample).
 // Gradient inputs: d rgb (required, or a target image for the fused MSE loss), d depth, d weights, d alpha,
 // d input_feat (optional) -- everything `rendering` returns is differentiable as in the reference.
-#include "render_frontend.cuh"
-#include "mlp_fp32.cuh"
+#include "tile_fp32.cuh"
 
 namespace mvsn {
 
@@ -83,20 +83,7 @@ struct BwdIO {
 
 namespace {
 
-// fragment <-> memory helpers.  Fragment of thread (ty, tx): rows {4ty+i, 64+4ty+i}, cols {4tx+j, 64+4tx+j}.
-__device__ __forceinline__ int frag_row(int ty, int r) { return (r < 4 ? 0 : 64) + ty * 4 + (r & 3); }
-__device__ __forceinline__ int frag_col(int tx, int n) { return (n < 4 ? 0 : 64) + tx * 4 + (n & 3); }
-
-// row-major [128][ld] store (shared or global)
-__device__ __forceinline__ void frag_store_rm(const float (&acc)[8][8], float* dst, int ld, int tid) {
-    const int ty = tid >> 4, tx = tid & 15;
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-        float* p = dst + frag_row(ty, r) * ld + tx * 4;
-        *reinterpret_cast<float4*>(p) = make_float4(acc[r][0], acc[r][1], acc[r][2], acc[r][3]);
-        *reinterpret_cast<float4*>(p + 64) = make_float4(acc[r][4], acc[r][5], acc[r][6], acc[r][7]);
-    }
-}
+// fragment <-> memory helpers of the backward (fragment layout: frag_row / frag_col in tile_fp32.cuh)
 // transposed store: dstT[col][row] with 128-float rows (global scratch)
 __device__ __forceinline__ void frag_store_T(const float (&acc)[8][8], float* dstT, int tid) {
     const int ty = tid >> 4, tx = tid & 15;
@@ -134,24 +121,6 @@ __device__ __forceinline__ void frag_accumulate(const float (&acc)[MR][NT], floa
         }
     }
 }
-// bias add (MODE 0) or relu((acc + bias) * mod) (MODE 1) in place; mod read from shared [128][H_LD]
-template <int MODE>
-__device__ __forceinline__ void epilogue128(float (&acc)[8][8], const float* __restrict__ bias, const float* s_mod, int tid) {
-    const int ty = tid >> 4, tx = tid & 15;
-    const float4 bl = __ldg(reinterpret_cast<const float4*>(bias + tx * 4));
-    const float4 bh = __ldg(reinterpret_cast<const float4*>(bias + 64 + tx * 4));
-    const float b[8] = {bl.x, bl.y, bl.z, bl.w, bh.x, bh.y, bh.z, bh.w};
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-        const int row = frag_row(ty, r);
-#pragma unroll
-        for (int n = 0; n < 8; ++n) {
-            float v = acc[r][n] + b[n];
-            if (MODE == 1) v = fmaxf(v * s_mod[row * H_LD + frag_col(tx, n)], 0.f);
-            acc[r][n] = v;
-        }
-    }
-}
 // [rows][128] dense global -> shared [rows][H_LD]
 __device__ __forceinline__ void stage_T(float* s_dst, const float* g_src, int rows, int tid) {
     for (int i = tid; i < rows * 32; i += 256) {
@@ -170,23 +139,27 @@ __device__ __forceinline__ void colsum_accumulate(const float* s_src, int ld, in
     }
 }
 
-constexpr int BWD_SMEM_FLOATS = TILE_M * PE_LD + 2 * TILE_M * H_LD + 2 * KCHUNK * 128 + TILE_M * 28;
+// What the backward keeps of the forward, in the CTA's scratch: the layer inputs and outputs transposed
+struct ScratchRecord {
+    float* scr;
+    __device__ __forceinline__ void pe(int row, int k, float v) const { scr[bwd::S_PET + k * 128 + row] = v; }
+    __device__ __forceinline__ void feat(int row, int k, float v) const { scr[bwd::S_FEATT + k * 128 + row] = v; }
+    __device__ __forceinline__ void mod(const float (&acc)[8][8], int tid) const { frag_store_T(acc, scr + bwd::S_MODT, tid); }
+    __device__ __forceinline__ void hidden(int l, const float (&acc)[8][8], int tid) const {
+        frag_store_T(acc, scr + bwd::S_HT + l * 16384, tid);
+    }
+    __device__ __forceinline__ void feature(const float (&acc)[8][8], int tid) const { frag_store_T(acc, scr + bwd::S_FT, tid); }
+};
+
+constexpr int BWD_SMEM_FLOATS = TILE_SMEM_FLOATS + TILE_M * 18;
 constexpr size_t BWD_SMEM_BYTES = BWD_SMEM_FLOATS * sizeof(float);
 static_assert(TILE_M * PE_LD >= 64 * H_LD, "peT staging [64][H_LD] must fit in the positional-encoding region");
 
 __global__ void __launch_bounds__(256, 1)
 render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts) {
     extern __shared__ __align__(16) float smem[];
-    float* s_pe   = smem;                          // forward: [128][PE_LD] ; backward: peT staged as [64][H_LD]
-    float* s_h    = s_pe + TILE_M * PE_LD;         // [128][H_LD]  forward activations ; backward: A operand (row-major)
-    float* s_mod  = s_h + TILE_M * H_LD;           // [128][H_LD]  modulation / hv ; backward: A operand (x^T)
-    float* s_w    = s_mod + TILE_M * H_LD;         // 2 x [32][128] streamed B chunks
-    float* s_misc = s_w + 2 * KCHUNK * 128;
-    float* s_dir  = s_misc;                        // [128][4] view direction
-    float* s_z    = s_dir + TILE_M * 4;            // [128]
-    float* s_sig  = s_z + TILE_M;                  // [128] sigma = relu(alpha_linear)
-    float* s_rgb  = s_sig + TILE_M;                // [128][4] r, g, b, alpha
-    float* s_T    = s_rgb + TILE_M * 4;            // [128] transmittance in front of the sample
+    const TileSmem sm(smem);                       // backward: sm.pe holds peT as [64][H_LD]; sm.h, sm.mod the A operands
+    float* s_T    = sm.tail;                       // [128] transmittance in front of the sample
     float* s_g    = s_T + TILE_M;                  // [128][4] d rgb_pre (3), d sigma_pre
     float* s_df   = s_g + TILE_M * 4;              // [128][8] d volume features ; [128][4] spare
     const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
@@ -205,139 +178,16 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
 
     for (int grp = blockIdx.x; grp < ngroups; grp += gridDim.x) {
         // =============================== forward recompute ===========================================
-        int r_in = 0, s_idx = 0;
         bool valid = false;
         size_t si = 0;
         if (tid < TILE_M) {
-            r_in = tid / S; s_idx = tid - r_in * S;
-            const int ray = grp * R + r_in;
+            const int r_in = tid / S, s_idx = tid - r_in * S, ray = grp * R + r_in;
             valid = r_in < R && ray < N;
-            float pe[3] = {0.f, 0.f, 0.f}, feat[20], dir[3] = {0.f, 0.f, 0.f}, zv = 0.f;
-#pragma unroll
-            for (int i = 0; i < 20; ++i) feat[i] = 0.f;
-            if (valid) {
-                si = (size_t)ray * S + s_idx;
-                const float px = __ldg(io.pts + si * 3), py = __ldg(io.pts + si * 3 + 1), pz = __ldg(io.pts + si * 3 + 2);
-                pe[0] = __ldg(io.ndc + si * 3); pe[1] = __ldg(io.ndc + si * 3 + 1); pe[2] = __ldg(io.ndc + si * 3 + 2);
-                zv = __ldg(io.z + si);
-                const float dx = __ldg(io.dirs + (size_t)ray * 3), dy = __ldg(io.dirs + (size_t)ray * 3 + 1),
-                            dz = __ldg(io.dirs + (size_t)ray * 3 + 2);
-                view_dir(cams, dx, dy, dz, dir);
-                sample_volume(sc, pe[0], pe[1], pe[2], feat);
-#pragma unroll
-                for (int v = 0; v < 3; ++v) sample_color(sc, cams, v, px, py, pz, feat + 8 + 4 * v);
-            }
-            float* pr = s_pe + tid * PE_LD;
-            float* peT = scr + bwd::S_PET + tid;
-            pr[0] = pe[0]; pr[1] = pe[1]; pr[2] = pe[2];
-            peT[0] = pe[0]; peT[128] = pe[1]; peT[256] = pe[2];
-            float f = 1.f;
-#pragma unroll
-            for (int k = 0; k < 10; ++k) {
-#pragma unroll
-                for (int j = 0; j < 3; ++j) {
-                    float sn, cs;
-                    sincosf(pe[j] * f, &sn, &cs);
-                    pr[3 + 3 * k + j] = sn; pr[33 + 3 * k + j] = cs;
-                    peT[(3 + 3 * k + j) * 128] = sn; peT[(33 + 3 * k + j) * 128] = cs;
-                }
-                f *= 2.f;
-            }
-            pr[63] = 0.f; peT[63 * 128] = 0.f;
-            float* fr = s_h + tid * FEAT_LD;
-            float* fT = scr + bwd::S_FEATT + tid;
-#pragma unroll
-            for (int i = 0; i < 32; ++i) { const float v = i < 20 ? feat[i] : 0.f; fr[i] = v; fT[i * 128] = v; }
-            s_dir[tid * 4 + 0] = dir[0]; s_dir[tid * 4 + 1] = dir[1]; s_dir[tid * 4 + 2] = dir[2];
-            s_z[tid] = zv;
+            si = (size_t)ray * S + s_idx;
+            tile_front_end<false>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr});
         }
         __syncthreads();
-        {
-            float acc[8][8];
-            zero_acc(acc);                                                     // modulation = pts_bias(feat)
-            gemm_pass<128>(acc, s_h, FEAT_LD, 32, wts + w32::WB, s_w, tid);
-            epilogue128<0>(acc, wts + w32::BB, nullptr, tid);
-            frag_store_rm(acc, s_mod, H_LD, tid);
-            frag_store_T(acc, scr + bwd::S_MODT, tid);
-            __syncthreads();
-            zero_acc(acc);                                                     // layer 0
-            gemm_pass<128>(acc, s_pe, PE_LD, 64, wts + w32::W0, s_w, tid);
-            epilogue128<1>(acc, wts + w32::B0, s_mod, tid);
-            frag_store_rm(acc, s_h, H_LD, tid);
-            frag_store_T(acc, scr + bwd::S_HT, tid);
-            __syncthreads();
-            for (int l = 0; l < 4; ++l) {                                      // layers 1..4
-                zero_acc(acc);
-                gemm_pass<128>(acc, s_h, H_LD, 128, wts + w32::W1 + l * w32::LSTR, s_w, tid);
-                epilogue128<1>(acc, wts + w32::W1 + l * w32::LSTR + 128 * 128, s_mod, tid);
-                frag_store_rm(acc, s_h, H_LD, tid);
-                frag_store_T(acc, scr + bwd::S_HT + (l + 1) * 16384, tid);
-                __syncthreads();
-            }
-            zero_acc(acc);                                                     // layer 5: [pe, h] -> 128
-            gemm_pass<128>(acc, s_pe, PE_LD, 64, wts + w32::W5, s_w, tid);
-            gemm_pass<128>(acc, s_h, H_LD, 128, wts + w32::W5 + 64 * 128, s_w, tid);
-            epilogue128<1>(acc, wts + w32::B5, s_mod, tid);
-            frag_store_rm(acc, s_h, H_LD, tid);
-            frag_store_T(acc, scr + bwd::S_HT + 5 * 16384, tid);
-            __syncthreads();
-            if (tid < TILE_M) {                                                // sigma = relu(alpha_linear(h6))
-                const float4* hr = reinterpret_cast<const float4*>(s_h + tid * H_LD);
-                const float4* wa = reinterpret_cast<const float4*>(wts + w32::WA);
-                float s = 0.f;
-#pragma unroll 8
-                for (int i = 0; i < 32; ++i) {
-                    const float4 a = hr[i], b = __ldg(wa + i);
-                    s = fmaf(a.x, b.x, s); s = fmaf(a.y, b.y, s); s = fmaf(a.z, b.z, s); s = fmaf(a.w, b.w, s);
-                }
-                s_sig[tid] = fmaxf(s + __ldg(wts + w32::BA), 0.f);
-            }
-            zero_acc(acc);                                                     // f = feature_linear(h6)
-            gemm_pass<128>(acc, s_h, H_LD, 128, wts + w32::WF, s_w, tid);
-            epilogue128<0>(acc, wts + w32::BF, nullptr, tid);
-            frag_store_rm(acc, s_h, H_LD, tid);
-            frag_store_T(acc, scr + bwd::S_FT, tid);
-            __syncthreads();
-        }
-        {
-            float acc[8][4];                                                   // hv = relu(views_linear([f, dir])) -> s_mod [128][HV_LD]
-            zero_acc(acc);
-            gemm_pass<64>(acc, s_h, H_LD, 128, wts + w32::WV, s_w, tid);
-            const float4 bv = __ldg(reinterpret_cast<const float4*>(wts + w32::BV + tx * 4));
-            const float4 wd0 = __ldg(reinterpret_cast<const float4*>(wts + w32::WVD + 0 * 64 + tx * 4));
-            const float4 wd1 = __ldg(reinterpret_cast<const float4*>(wts + w32::WVD + 1 * 64 + tx * 4));
-            const float4 wd2 = __ldg(reinterpret_cast<const float4*>(wts + w32::WVD + 2 * 64 + tx * 4));
-#pragma unroll
-            for (int r = 0; r < 8; ++r) {
-                const int row = frag_row(ty, r);
-                const float d0 = s_dir[row * 4], d1 = s_dir[row * 4 + 1], d2 = s_dir[row * 4 + 2];
-                float4 o;
-                o.x = fmaxf(fmaf(d2, wd2.x, fmaf(d1, wd1.x, fmaf(d0, wd0.x, acc[r][0]))) + bv.x, 0.f);
-                o.y = fmaxf(fmaf(d2, wd2.y, fmaf(d1, wd1.y, fmaf(d0, wd0.y, acc[r][1]))) + bv.y, 0.f);
-                o.z = fmaxf(fmaf(d2, wd2.z, fmaf(d1, wd1.z, fmaf(d0, wd0.z, acc[r][2]))) + bv.z, 0.f);
-                o.w = fmaxf(fmaf(d2, wd2.w, fmaf(d1, wd1.w, fmaf(d0, wd0.w, acc[r][3]))) + bv.w, 0.f);
-                *reinterpret_cast<float4*>(s_mod + row * HV_LD + tx * 4) = o;
-            }
-            __syncthreads();
-        }
-        if (tid < TILE_M) {                                                    // rgb = sigmoid(rgb_linear(hv)), alpha
-            const float4* hr = reinterpret_cast<const float4*>(s_mod + tid * HV_LD);
-            float o[3];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float4* wr = reinterpret_cast<const float4*>(wts + w32::WR + c * 64);
-                float s = 0.f;
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float4 a = hr[i], b = __ldg(wr + i);
-                    s = fmaf(a.x, b.x, s); s = fmaf(a.y, b.y, s); s = fmaf(a.z, b.z, s); s = fmaf(a.w, b.w, s);
-                }
-                s += __ldg(wts + w32::BR + c);
-                o[c] = __fdiv_rn(1.f, 1.f + expf(-s));
-            }
-            s_rgb[tid * 4 + 0] = o[0]; s_rgb[tid * 4 + 1] = o[1]; s_rgb[tid * 4 + 2] = o[2];
-            s_rgb[tid * 4 + 3] = 1.f - expf(-s_sig[tid]);
-        }
+        tile_mlp(sm, wts, tid, ScratchRecord{scr});
         __syncthreads();
 
         // =============================== compositing: forward + reverse scan ===========================
@@ -348,10 +198,10 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
             if (ray < N) {
                 float cr = 0.f, cg = 0.f, cb = 0.f, dp = 0.f, ac = 0.f, T = 1.f;
                 for (int j = first; j < first + S; ++j) {
-                    const float a = s_rgb[j * 4 + 3], w = a * T;
+                    const float a = sm.rgb[j * 4 + 3], w = a * T;
                     s_T[j] = T;
-                    cr = fmaf(w, s_rgb[j * 4 + 0], cr); cg = fmaf(w, s_rgb[j * 4 + 1], cg); cb = fmaf(w, s_rgb[j * 4 + 2], cb);
-                    dp = fmaf(w, s_z[j], dp); ac += w;
+                    cr = fmaf(w, sm.rgb[j * 4 + 0], cr); cg = fmaf(w, sm.rgb[j * 4 + 1], cg); cb = fmaf(w, sm.rgb[j * 4 + 2], cb);
+                    dp = fmaf(w, sm.z[j], dp); ac += w;
                     T *= (1.f - a) + 1e-10f;
                 }
                 if (sc.white_bkgd) { const float bg = 1.f - ac; cr += bg; cg += bg; cb += bg; }
@@ -371,9 +221,9 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
                 float B = 0.f;
                 for (int j = first + S - 1; j >= first; --j) {
                     const size_t sj = (size_t)ray * S + (j - first);
-                    const float a = s_rgb[j * 4 + 3], Tj = s_T[j], w = a * Tj;
-                    const float c0 = s_rgb[j * 4], c1 = s_rgb[j * 4 + 1], c2 = s_rgb[j * 4 + 2];
-                    float dw = g0 * c0 + g1 * c1 + g2 * c2 + gd * s_z[j] - gbg;
+                    const float a = sm.rgb[j * 4 + 3], Tj = s_T[j], w = a * Tj;
+                    const float c0 = sm.rgb[j * 4], c1 = sm.rgb[j * 4 + 1], c2 = sm.rgb[j * 4 + 2];
+                    float dw = g0 * c0 + g1 * c1 + g2 * c2 + gd * sm.z[j] - gbg;
                     if (bw.g_weights) dw += __ldg(bw.g_weights + sj);
                     float da = Tj * (dw - B);
                     if (bw.g_alpha) da += __ldg(bw.g_alpha + sj);
@@ -381,14 +231,14 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
                     s_g[j * 4 + 0] = w * g0 * c0 * (1.f - c0);
                     s_g[j * 4 + 1] = w * g1 * c1 * (1.f - c1);
                     s_g[j * 4 + 2] = w * g2 * c2 * (1.f - c2);
-                    s_g[j * 4 + 3] = s_sig[j] > 0.f ? da * (1.f - a) : 0.f;
+                    s_g[j * 4 + 3] = sm.sig[j] > 0.f ? da * (1.f - a) : 0.f;
                 }
             } else {
                 for (int j = first; j < first + S; ++j) { s_g[j * 4] = s_g[j * 4 + 1] = s_g[j * 4 + 2] = s_g[j * 4 + 3] = 0.f; }
             }
         }
         if (tid >= R * S && tid < TILE_M) { s_g[tid * 4] = s_g[tid * 4 + 1] = s_g[tid * 4 + 2] = s_g[tid * 4 + 3] = 0.f; }
-        stage_T(s_pe, scr + bwd::S_PET, 64, tid);             // peT -> shared (used by the layer-5 and layer-0 wgrads)
+        stage_T(sm.pe, scr + bwd::S_PET, 64, tid);             // peT -> shared (used by the layer-5 and layer-0 wgrads)
         __syncthreads();
 
         // =============================== backward through the heads =================================
@@ -396,7 +246,7 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
         if (tid < 64) {
             float a0 = 0.f, a1 = 0.f, a2 = 0.f;
             for (int r = 0; r < TILE_M; ++r) {
-                const float h = s_mod[r * HV_LD + tid];
+                const float h = sm.mod[r * HV_LD + tid];
                 a0 = fmaf(s_g[r * 4], h, a0); a1 = fmaf(s_g[r * 4 + 1], h, a1); a2 = fmaf(s_g[r * 4 + 2], h, a2);
             }
             G[bwd::G_WR + tid] += a0; G[bwd::G_WR + 64 + tid] += a1; G[bwd::G_WR + 128 + tid] += a2;
@@ -407,7 +257,7 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
             G[bwd::G_BR + c] += a;                             // c == 3: d ba = sum d sigma_pre
         }
         {
-            // d hv_pre[r][j] = (hv > 0) * sum_c d rgb_pre[r][c] Wr[c][j]   -> s_h (A, lda H_LD) and scratch [128][64] (B)
+            // d hv_pre[r][j] = (hv > 0) * sum_c d rgb_pre[r][c] Wr[c][j]   -> sm.h (A, lda H_LD) and scratch [128][64] (B)
             const float4 w0 = __ldg(reinterpret_cast<const float4*>(wts + w32::WR + tx * 4));
             const float4 w1 = __ldg(reinterpret_cast<const float4*>(wts + w32::WR + 64 + tx * 4));
             const float4 w2 = __ldg(reinterpret_cast<const float4*>(wts + w32::WR + 128 + tx * 4));
@@ -415,23 +265,23 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
             for (int r = 0; r < 8; ++r) {
                 const int row = frag_row(ty, r);
                 const float d0 = s_g[row * 4], d1 = s_g[row * 4 + 1], d2 = s_g[row * 4 + 2];
-                const float4 hv = *reinterpret_cast<const float4*>(s_mod + row * HV_LD + tx * 4);
+                const float4 hv = *reinterpret_cast<const float4*>(sm.mod + row * HV_LD + tx * 4);
                 float4 o;
                 o.x = hv.x > 0.f ? fmaf(d2, w2.x, fmaf(d1, w1.x, d0 * w0.x)) : 0.f;
                 o.y = hv.y > 0.f ? fmaf(d2, w2.y, fmaf(d1, w1.y, d0 * w0.y)) : 0.f;
                 o.z = hv.z > 0.f ? fmaf(d2, w2.z, fmaf(d1, w1.z, d0 * w0.z)) : 0.f;
                 o.w = hv.w > 0.f ? fmaf(d2, w2.w, fmaf(d1, w1.w, d0 * w0.w)) : 0.f;
-                *reinterpret_cast<float4*>(s_h + row * H_LD + tx * 4) = o;
+                *reinterpret_cast<float4*>(sm.h + row * H_LD + tx * 4) = o;
                 *reinterpret_cast<float4*>(scr + bwd::S_DPRE + row * 64 + tx * 4) = o;
             }
         }
-        __syncthreads();                                        // hv (s_mod) no longer needed; d hv_pre complete
-        stage_T(s_mod, scr + bwd::S_FT, 128, tid);              // fT -> A operand of the views wgrad
+        __syncthreads();                                        // hv (sm.mod) no longer needed; d hv_pre complete
+        stage_T(sm.mod, scr + bwd::S_FT, 128, tid);              // fT -> A operand of the views wgrad
         if (tid < 64) {                                         // d bv, d Wv[:, 128:131]^T
             float sb = 0.f, s0 = 0.f, s1 = 0.f, s2 = 0.f;
             for (int r = 0; r < TILE_M; ++r) {
-                const float d = s_h[r * H_LD + tid];
-                sb += d; s0 = fmaf(s_dir[r * 4], d, s0); s1 = fmaf(s_dir[r * 4 + 1], d, s1); s2 = fmaf(s_dir[r * 4 + 2], d, s2);
+                const float d = sm.h[r * H_LD + tid];
+                sb += d; s0 = fmaf(sm.dir[r * 4], d, s0); s1 = fmaf(sm.dir[r * 4 + 1], d, s1); s2 = fmaf(sm.dir[r * 4 + 2], d, s2);
             }
             G[bwd::G_BV + tid] += sb;
             G[bwd::G_WVDT + tid] += s0; G[bwd::G_WVDT + 64 + tid] += s1; G[bwd::G_WVDT + 128 + tid] += s2;
@@ -441,29 +291,29 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
         {
             float acc[8][4];                                    // d Wv_f^T[k][j] = sum_r fT[k][r] d hv_pre[r][j]
             zero_acc(acc);
-            gemm_pass<64>(acc, s_mod, H_LD, 128, scr + bwd::S_DPRE, s_w, tid);
+            gemm_pass<64>(acc, sm.mod, H_LD, 128, scr + bwd::S_DPRE, sm.w, tid);
             frag_accumulate(acc, G + bwd::G_WVFT, 64, tid);
         }
         float acc[8][8];
         zero_acc(acc);                                          // d f[r][k] = sum_j d hv_pre[r][j] Wv[j][k]
-        gemm_pass<128>(acc, s_h, H_LD, 64, bw.wd + bwd::D_VF, s_w, tid);
-        frag_store_rm(acc, s_h, H_LD, tid);
+        gemm_pass<128>(acc, sm.h, H_LD, 64, bw.wd + bwd::D_VF, sm.w, tid);
+        frag_store_rm(acc, sm.h, H_LD, tid);
         frag_store_rm(acc, scr + bwd::S_DPRE, 128, tid);
         __syncthreads();
-        stage_T(s_mod, scr + bwd::S_HT + 5 * 16384, 128, tid);  // h6T
-        colsum_accumulate(s_h, H_LD, 128, G + bwd::G_BF, tid);  // d bf
+        stage_T(sm.mod, scr + bwd::S_HT + 5 * 16384, 128, tid);  // h6T
+        colsum_accumulate(sm.h, H_LD, 128, G + bwd::G_BF, tid);  // d bf
         cp_async_wait<0>();
         __syncthreads();
         zero_acc(acc);                                          // d Wf^T[k][n] = sum_r h6T[k][r] d f[r][n]
-        gemm_pass<128>(acc, s_mod, H_LD, 128, scr + bwd::S_DPRE, s_w, tid);
+        gemm_pass<128>(acc, sm.mod, H_LD, 128, scr + bwd::S_DPRE, sm.w, tid);
         frag_accumulate(acc, G + bwd::G_WFT, 128, tid);
         if (tid < TILE_M) {                                     // d wa[k] = sum_r d sigma_pre[r] h6T[k][r]
             float s = 0.f;
-            for (int r = 0; r < TILE_M; ++r) s = fmaf(s_g[r * 4 + 3], s_mod[tid * H_LD + r], s);
+            for (int r = 0; r < TILE_M; ++r) s = fmaf(s_g[r * 4 + 3], sm.mod[tid * H_LD + r], s);
             G[bwd::G_WA + tid] += s;
         }
         zero_acc(acc);                                          // d h6 = d f Wf + d sigma_pre (x) wa
-        gemm_pass<128>(acc, s_h, H_LD, 128, bw.wd + bwd::D_F, s_w, tid);
+        gemm_pass<128>(acc, sm.h, H_LD, 128, bw.wd + bwd::D_F, sm.w, tid);
         {
             const float4 al = __ldg(reinterpret_cast<const float4*>(wts + w32::WA + tx * 4));
             const float4 ah = __ldg(reinterpret_cast<const float4*>(wts + w32::WA + 64 + tx * 4));
@@ -507,48 +357,48 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
                     }
                 }
             }
-            frag_store_rm(acc, s_h, H_LD, tid);
+            frag_store_rm(acc, sm.h, H_LD, tid);
             frag_store_rm(acc, scr + bwd::S_DPRE, 128, tid);
             __syncthreads();
-            if (l >= 1) stage_T(s_mod, scr + bwd::S_HT + (l - 1) * 16384, 128, tid);      // x_l^T = h_l^T
-            colsum_accumulate(s_h, H_LD, 128, G + bwd::G_B + l * 128, tid);                // d b_l
+            if (l >= 1) stage_T(sm.mod, scr + bwd::S_HT + (l - 1) * 16384, 128, tid);      // x_l^T = h_l^T
+            colsum_accumulate(sm.h, H_LD, 128, G + bwd::G_B + l * 128, tid);                // d b_l
             cp_async_wait<0>();
             __syncthreads();
             if (l >= 1) {                                       // d W_l^T[k][n] = sum_r h_l^T[k][r] d pre[r][n]
                 zero_acc(acc);
-                gemm_pass<128>(acc, s_mod, H_LD, 128, scr + bwd::S_DPRE, s_w, tid);
+                gemm_pass<128>(acc, sm.mod, H_LD, 128, scr + bwd::S_DPRE, sm.w, tid);
                 frag_accumulate(acc, G + (l == 5 ? bwd::G_W5HT : bwd::G_W14T + (l - 1) * 16384), 128, tid);
             }
             if (l == 5 || l == 0) {                             // positional-encoding part: 64-row A
                 float a4[4][8];
                 zero_acc(a4);
-                gemm_pass<128>(a4, s_pe, H_LD, 128, scr + bwd::S_DPRE, s_w, tid);
+                gemm_pass<128>(a4, sm.pe, H_LD, 128, scr + bwd::S_DPRE, sm.w, tid);
                 frag_accumulate(a4, G + (l == 5 ? bwd::G_W5PET : bwd::G_W0T), 128, tid);
             }
             if (l >= 1) {                                       // d h_l = d pre W_l (h part)
                 zero_acc(acc);
-                gemm_pass<128>(acc, s_h, H_LD, 128, bw.wd + (l == 5 ? bwd::D_5H : bwd::D_14 + (l - 1) * 16384), s_w, tid);
+                gemm_pass<128>(acc, sm.h, H_LD, 128, bw.wd + (l == 5 ? bwd::D_5H : bwd::D_14 + (l - 1) * 16384), sm.w, tid);
             }
         }
         // =============================== modulation branch: pts_bias ==================================
         // d mod is complete in scratch (transposed): bring it to row-major -- A operand of d feat (shared), B operand of d Wb
         frag_load_T(acc, scr + bwd::S_DMOD, tid);
-        frag_store_rm(acc, s_h, H_LD, tid);
+        frag_store_rm(acc, sm.h, H_LD, tid);
         frag_store_rm(acc, scr + bwd::S_DPRE, 128, tid);
-        stage_T(s_mod, scr + bwd::S_FEATT, 64, tid);
+        stage_T(sm.mod, scr + bwd::S_FEATT, 64, tid);
         cp_async_wait<0>();
         __syncthreads();
-        colsum_accumulate(s_h, H_LD, 128, G + bwd::G_BB, tid);
+        colsum_accumulate(sm.h, H_LD, 128, G + bwd::G_BB, tid);
         {
             float a4[4][8];                                     // d Wb^T[k][n] = sum_r featT[k][r] d mod[r][n]
             zero_acc(a4);
-            gemm_pass<128>(a4, s_mod, H_LD, 128, scr + bwd::S_DPRE, s_w, tid);
+            gemm_pass<128>(a4, sm.mod, H_LD, 128, scr + bwd::S_DPRE, sm.w, tid);
             frag_accumulate(a4, G + bwd::G_WBT, 128, tid);
         }
         if (bw.dvol) {
             float a[8][4];                                      // d feat[r][k] = sum_n d mod[r][n] Wb[n][k]
             zero_acc(a);
-            gemm_pass<64>(a, s_h, H_LD, 128, bw.wd + bwd::D_B, s_w, tid);
+            gemm_pass<64>(a, sm.h, H_LD, 128, bw.wd + bwd::D_B, sm.w, tid);
             if (tx < 2) {
 #pragma unroll
                 for (int r = 0; r < 8; ++r)
@@ -564,20 +414,13 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
 #pragma unroll
                     for (int c = 0; c < 8; ++c) g8[c] += __ldg(bw.g_feat + si * 20 + c);
                 }
-                const float nx = __ldg(io.ndc + si * 3), ny = __ldg(io.ndc + si * 3 + 1), nz = __ldg(io.ndc + si * 3 + 2);
+                const Trilinear t = trilinear_corners(sc, __ldg(io.ndc + si * 3), __ldg(io.ndc + si * 3 + 1), __ldg(io.ndc + si * 3 + 2));
                 const int W = sc.Wp, H = sc.Hp, D = sc.D;
-                const float ix = ((nx * 2.f - 1.f + 1.f) * 0.5f) * (float)(W - 1);
-                const float iy = ((ny * 2.f - 1.f + 1.f) * 0.5f) * (float)(H - 1);
-                const float iz = ((nz * 2.f - 1.f + 1.f) * 0.5f) * (float)(D - 1);
-                const float x0f = floorf(ix), y0f = floorf(iy), z0f = floorf(iz);
-                const float wx[2] = {(x0f + 1.f) - ix, ix - x0f}, wy[2] = {(y0f + 1.f) - iy, iy - y0f}, wz[2] = {(z0f + 1.f) - iz, iz - z0f};
-                const int x0 = (int)fminf(fmaxf(x0f, -2.f), (float)W), y0 = (int)fminf(fmaxf(y0f, -2.f), (float)H),
-                          z0 = (int)fminf(fmaxf(z0f, -2.f), (float)D);
 #pragma unroll
                 for (int c = 0; c < 8; ++c) {
-                    const int x = x0 + (c & 1), y = y0 + ((c >> 1) & 1), z = z0 + (c >> 2);
-                    if ((unsigned)x >= (unsigned)W || (unsigned)y >= (unsigned)H || (unsigned)z >= (unsigned)D) continue;
-                    const float wgt = wx[c & 1] * wy[(c >> 1) & 1] * wz[c >> 2];
+                    const int x = t.x0 + (c & 1), y = t.y0 + ((c >> 1) & 1), z = t.z0 + (c >> 2);
+                    if ((unsigned)x >= (unsigned)W || (unsigned)y >= (unsigned)H || (unsigned)z >= (unsigned)D) continue;   // zeros padding
+                    const float wgt = t.wx[c & 1] * t.wy[(c >> 1) & 1] * t.wz[c >> 2];
                     float4* p = reinterpret_cast<float4*>(bw.dvol + (((size_t)z * H + y) * W + x) * 8);
                     atomicAdd(p, make_float4(g8[0] * wgt, g8[1] * wgt, g8[2] * wgt, g8[3] * wgt));
                     atomicAdd(p + 1, make_float4(g8[4] * wgt, g8[5] * wgt, g8[6] * wgt, g8[7] * wgt));

@@ -8,31 +8,23 @@
 //              weights streamed L2 -> smem in 32-row chunks with cp.async double buffering,
 //              modulation / bias / activation fused into each pass epilogue
 //   back end   alpha compositing in shared memory, one 16-byte result per ray to HBM.
+// Front end and MLP are the fp32 forward tile (tile_fp32.cuh) the fine-tuning backward recomputes.
 // No per-sample value ever goes to HBM unless the caller asks for the optional outputs.
 //
 // Replaces renderer.rendering (renderer.py:138-165) and callees; see include/mvsnerf_b200.h.
-#include "render_frontend.cuh"
-#include "mlp_fp32.cuh"
+#include "tile_fp32.cuh"
 
 namespace mvsn {
 
-constexpr int SMEM_FLOATS = TILE_M * PE_LD + 2 * TILE_M * H_LD + 2 * KCHUNK * 128 + TILE_M * 12;
+constexpr int SMEM_FLOATS = TILE_SMEM_FLOATS + TILE_M * 2;
 constexpr size_t SMEM_BYTES = SMEM_FLOATS * sizeof(float);
 
 template <bool FAST>
 __global__ void __launch_bounds__(256, 1)
 render_fp32_kernel(const SceneDev sc, const RenderIO io, const float* __restrict__ wts) {
     extern __shared__ __align__(16) float smem[];
-    float* s_pe   = smem;                          // [128][PE_LD]
-    float* s_h    = s_pe + TILE_M * PE_LD;         // [128][H_LD]   (feat staging / h / f)
-    float* s_mod  = s_h + TILE_M * H_LD;           // [128][H_LD]   (modulation, later hv)
-    float* s_w    = s_mod + TILE_M * H_LD;         // 2 x [32][128] weight chunks
-    float* s_misc = s_w + 2 * KCHUNK * 128;        // per-row scalars
-    float* s_dir  = s_misc;                        // [128][4] view direction of the row's ray
-    float* s_z    = s_misc + TILE_M * 4;           // [128]
-    float* s_sig  = s_z + TILE_M;                  // [128] sigma, later 1-alpha+1e-10
-    float* s_rgb  = s_sig + TILE_M;                // [128][4] r,g,b,weight
-    float* s_carry = s_rgb + TILE_M * 4;           // [8]: T carry, rgb/depth/acc partial sums (S > 128)
+    const TileSmem sm(smem);
+    float* s_carry = sm.tail;                      // [8]: T carry, rgb/depth/acc partial sums (S > 128)
 
     const int tid = threadIdx.x;
     __shared__ Cams cams;
@@ -45,178 +37,31 @@ render_fp32_kernel(const SceneDev sc, const RenderIO io, const float* __restrict
 
     for (int grp = blockIdx.x; grp < ngroups; grp += gridDim.x) {
         for (int chunk = 0; chunk < nchunks; ++chunk) {
-            // ------------------------------ front end -------------------------------------
             int r_in = 0, s_idx = 0;
             bool valid = false;
             if (tid < TILE_M) {
                 if (S <= TILE_M) { r_in = tid / S; s_idx = tid - r_in * S; valid = r_in < R; }
                 else { r_in = 0; s_idx = chunk * TILE_M + tid; valid = s_idx < S; }
-                const int ray = grp * R + r_in;
-                valid = valid && ray < N;
-                float pe[3] = {0.f, 0.f, 0.f}, feat[20], dir[3] = {0.f, 0.f, 0.f}, zv = 0.f;
-#pragma unroll
-                for (int i = 0; i < 20; ++i) feat[i] = 0.f;
-                if (valid) {
-                    float px, py, pz, dx, dy, dz;
-                    const size_t si = (size_t)ray * S + s_idx;
-                    if (FAST) {
-                        const float4* rp = reinterpret_cast<const float4*>(io.rays + (size_t)ray * 8);
-                        float4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
-                        dx = r0.w; dy = r1.x; dz = r1.y;
-                        const float near = r1.z, far = r1.w, t = __ldg(io.t_steps + s_idx);
-                        if (!io.rg.lindisp) zv = __fadd_rn(__fmul_rn(near, 1.f - t), __fmul_rn(far, t));
-                        else zv = __fdiv_rn(1.f, __fadd_rn(__fmul_rn(__fdiv_rn(1.f, near), 1.f - t),
-                                                           __fmul_rn(__fdiv_rn(1.f, far), t)));
-                        px = __fadd_rn(r0.x, __fmul_rn(dx, zv));
-                        py = __fadd_rn(r0.y, __fmul_rn(dy, zv));
-                        pz = __fadd_rn(r0.z, __fmul_rn(dz, zv));
-                        ndc_of_point(sc, cams, io.rg, px, py, pz, pe[0], pe[1], pe[2]);
-                    } else {
-                        px = __ldg(io.pts + si * 3); py = __ldg(io.pts + si * 3 + 1); pz = __ldg(io.pts + si * 3 + 2);
-                        pe[0] = __ldg(io.ndc + si * 3); pe[1] = __ldg(io.ndc + si * 3 + 1); pe[2] = __ldg(io.ndc + si * 3 + 2);
-                        zv = __ldg(io.z + si);
-                        dx = __ldg(io.dirs + (size_t)ray * 3); dy = __ldg(io.dirs + (size_t)ray * 3 + 1);
-                        dz = __ldg(io.dirs + (size_t)ray * 3 + 2);
-                    }
-                    view_dir(cams, dx, dy, dz, dir);
-                    sample_volume(sc, pe[0], pe[1], pe[2], feat);
-#pragma unroll
-                    for (int v = 0; v < 3; ++v) sample_color(sc, cams, v, px, py, pz, feat + 8 + 4 * v);
-                    if (io.input_feat) {
-                        float4* o = reinterpret_cast<float4*>(io.input_feat + si * 20);
-#pragma unroll
-                        for (int i = 0; i < 5; ++i)
-                            o[i] = make_float4(feat[4 * i], feat[4 * i + 1], feat[4 * i + 2], feat[4 * i + 3]);
-                    }
-                }
-                // positional encoding (models.py:47-51): [x, sin(2^k x) k-major, cos(2^k x) k-major]
-                float* pr = s_pe + tid * PE_LD;
-                pr[0] = pe[0]; pr[1] = pe[1]; pr[2] = pe[2];
-                float f = 1.f;
-#pragma unroll
-                for (int k = 0; k < 10; ++k) {
-#pragma unroll
-                    for (int j = 0; j < 3; ++j) {
-                        float sn, cs;
-                        sincosf(pe[j] * f, &sn, &cs);
-                        pr[3 + 3 * k + j] = sn;
-                        pr[33 + 3 * k + j] = cs;
-                    }
-                    f *= 2.f;
-                }
-                pr[63] = 0.f;
-                float* fr = s_h + tid * FEAT_LD;
-#pragma unroll
-                for (int i = 0; i < 20; ++i) fr[i] = feat[i];
-#pragma unroll
-                for (int i = 20; i < 32; ++i) fr[i] = 0.f;
-                s_dir[tid * 4 + 0] = dir[0]; s_dir[tid * 4 + 1] = dir[1]; s_dir[tid * 4 + 2] = dir[2];
-                s_z[tid] = zv;
+                valid = valid && grp * R + r_in < N;
+                tile_front_end<FAST>(sc, cams, io, sm, tid, grp * R + r_in, s_idx, valid, NoRecord{});
             }
             __syncthreads();
-
-            // ------------------------------ MLP (models.py:194-222) -----------------------
-            {
-                float acc[8][8];
-                // modulation = pts_bias(feat)
-                zero_acc(acc);
-                gemm_pass<128>(acc, s_h, FEAT_LD, 32, wts + w32::WB, s_w, tid);
-                store_pass128<0>(acc, wts + w32::BB, nullptr, s_mod, tid);
-                __syncthreads();
-                // layer 0: 63 -> 128
-                zero_acc(acc);
-                gemm_pass<128>(acc, s_pe, PE_LD, 64, wts + w32::W0, s_w, tid);
-                store_pass128<1>(acc, wts + w32::B0, s_mod, s_h, tid);
-                __syncthreads();
-                // layers 1..4: 128 -> 128
-                for (int l = 0; l < 4; ++l) {
-                    zero_acc(acc);
-                    gemm_pass<128>(acc, s_h, H_LD, 128, wts + w32::W1 + l * w32::LSTR, s_w, tid);
-                    store_pass128<1>(acc, wts + w32::W1 + l * w32::LSTR + 128 * 128, s_mod, s_h, tid);
-                    __syncthreads();
-                }
-                // layer 5: [pe63, h128] -> 128  (skip connection, models.py:204-205)
-                zero_acc(acc);
-                gemm_pass<128>(acc, s_pe, PE_LD, 64, wts + w32::W5, s_w, tid);
-                gemm_pass<128>(acc, s_h, H_LD, 128, wts + w32::W5 + 64 * 128, s_w, tid);
-                store_pass128<1>(acc, wts + w32::B5, s_mod, s_h, tid);
-                __syncthreads();
-                // sigma = relu(alpha_linear(h))
-                if (tid < TILE_M) {
-                    const float4* hr = reinterpret_cast<const float4*>(s_h + tid * H_LD);
-                    const float4* wa = reinterpret_cast<const float4*>(wts + w32::WA);
-                    float s = 0.f;
-#pragma unroll 8
-                    for (int i = 0; i < 32; ++i) {
-                        float4 a = hr[i], b = __ldg(wa + i);
-                        s = fmaf(a.x, b.x, s); s = fmaf(a.y, b.y, s); s = fmaf(a.z, b.z, s); s = fmaf(a.w, b.w, s);
-                    }
-                    s_sig[tid] = fmaxf(s + __ldg(wts + w32::BA), 0.f);
-                }
-                // feature = feature_linear(h)  (in place)
-                zero_acc(acc);
-                gemm_pass<128>(acc, s_h, H_LD, 128, wts + w32::WF, s_w, tid);
-                store_pass128<0>(acc, wts + w32::BF, nullptr, s_h, tid);
-                __syncthreads();
-            }
-            {
-                // views layer: relu(W [feature, dir] + b) : 131 -> 64 ; stored in the s_mod region
-                float acc[8][4];
-                zero_acc(acc);
-                gemm_pass<64>(acc, s_h, H_LD, 128, wts + w32::WV, s_w, tid);
-                const int ty = tid >> 4, tx = tid & 15;
-                float4 bv = __ldg(reinterpret_cast<const float4*>(wts + w32::BV + tx * 4));
-                float4 wd0 = __ldg(reinterpret_cast<const float4*>(wts + w32::WVD + 0 * 64 + tx * 4));
-                float4 wd1 = __ldg(reinterpret_cast<const float4*>(wts + w32::WVD + 1 * 64 + tx * 4));
-                float4 wd2 = __ldg(reinterpret_cast<const float4*>(wts + w32::WVD + 2 * 64 + tx * 4));
-#pragma unroll
-                for (int r = 0; r < 8; ++r) {
-                    int row = (r < 4 ? 0 : 64) + ty * 4 + (r & 3);
-                    float d0 = s_dir[row * 4], d1 = s_dir[row * 4 + 1], d2 = s_dir[row * 4 + 2];
-                    float4 o;
-                    o.x = fmaxf(fmaf(d2, wd2.x, fmaf(d1, wd1.x, fmaf(d0, wd0.x, acc[r][0]))) + bv.x, 0.f);
-                    o.y = fmaxf(fmaf(d2, wd2.y, fmaf(d1, wd1.y, fmaf(d0, wd0.y, acc[r][1]))) + bv.y, 0.f);
-                    o.z = fmaxf(fmaf(d2, wd2.z, fmaf(d1, wd1.z, fmaf(d0, wd0.z, acc[r][2]))) + bv.z, 0.f);
-                    o.w = fmaxf(fmaf(d2, wd2.w, fmaf(d1, wd1.w, fmaf(d0, wd0.w, acc[r][3]))) + bv.w, 0.f);
-                    *reinterpret_cast<float4*>(s_mod + row * HV_LD + tx * 4) = o;
-                }
-                __syncthreads();
-            }
-            // rgb = sigmoid(rgb_linear(hv)) ; alpha = 1 - exp(-sigma)   (renderer.py:18-26)
-            if (tid < TILE_M) {
-                const float4* hr = reinterpret_cast<const float4*>(s_mod + tid * HV_LD);
-                float o[3];
-#pragma unroll
-                for (int c = 0; c < 3; ++c) {
-                    const float4* wr = reinterpret_cast<const float4*>(wts + w32::WR + c * 64);
-                    float s = 0.f;
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        float4 a = hr[i], b = __ldg(wr + i);
-                        s = fmaf(a.x, b.x, s); s = fmaf(a.y, b.y, s); s = fmaf(a.z, b.z, s); s = fmaf(a.w, b.w, s);
-                    }
-                    s += __ldg(wts + w32::BR + c);
-                    o[c] = __fdiv_rn(1.f, 1.f + expf(-s));
-                }
-                s_rgb[tid * 4 + 0] = o[0]; s_rgb[tid * 4 + 1] = o[1]; s_rgb[tid * 4 + 2] = o[2];
-                const float a = 1.f - expf(-s_sig[tid]);
-                s_rgb[tid * 4 + 3] = a;                       // alpha (becomes the weight below)
-                s_sig[tid] = (1.f - a) + 1e-10f;              // transmittance factor
-            }
+            tile_mlp(sm, wts, tid, NoRecord{});
+            if (tid < TILE_M) sm.sig[tid] = (1.f - sm.rgb[tid * 4 + 3]) + 1e-10f;   // sigma -> transmittance factor
             __syncthreads();
 
             // ------------------------------ compositing (renderer.py:65-92) ----------------
             if (tid < TILE_M && valid) {
                 const int first = tid - (S <= TILE_M ? s_idx : tid);   // first row of this ray in the tile
                 float T = (chunk == 0) ? 1.f : s_carry[0];
-                for (int j = first; j < tid; ++j) T *= s_sig[j];
-                const float a = s_rgb[tid * 4 + 3];
+                for (int j = first; j < tid; ++j) T *= sm.sig[j];
+                const float a = sm.rgb[tid * 4 + 3];
                 const float w = a * T;
                 const size_t si = (size_t)(grp * R + r_in) * S + s_idx;
                 if (io.alpha) io.alpha[si] = a;
                 if (io.weights) io.weights[si] = w;
-                s_z[tid] *= w;                                 // depth contribution
-                s_rgb[tid * 4 + 3] = w;
+                sm.z[tid] *= w;                                // depth contribution
+                sm.rgb[tid * 4 + 3] = w;
             }
             __syncthreads();
             if (tid < R && grp * R + tid < N) {
@@ -226,10 +71,10 @@ render_fp32_kernel(const SceneDev sc, const RenderIO io, const float* __restrict
                 float cr = 0.f, cg = 0.f, cb = 0.f, dp = 0.f, ac = 0.f, T = 1.f;
                 if (chunk > 0) { T = s_carry[0]; cr = s_carry[1]; cg = s_carry[2]; cb = s_carry[3]; dp = s_carry[4]; ac = s_carry[5]; }
                 for (int j = first; j < first + cnt; ++j) {
-                    const float w = s_rgb[j * 4 + 3];
-                    cr = fmaf(w, s_rgb[j * 4 + 0], cr); cg = fmaf(w, s_rgb[j * 4 + 1], cg);
-                    cb = fmaf(w, s_rgb[j * 4 + 2], cb);
-                    dp += s_z[j]; ac += w; T *= s_sig[j];
+                    const float w = sm.rgb[j * 4 + 3];
+                    cr = fmaf(w, sm.rgb[j * 4 + 0], cr); cg = fmaf(w, sm.rgb[j * 4 + 1], cg);
+                    cb = fmaf(w, sm.rgb[j * 4 + 2], cb);
+                    dp += sm.z[j]; ac += w; T *= sm.sig[j];
                 }
                 if (chunk + 1 < nchunks) {
                     s_carry[0] = T; s_carry[1] = cr; s_carry[2] = cg; s_carry[3] = cb; s_carry[4] = dp; s_carry[5] = ac;

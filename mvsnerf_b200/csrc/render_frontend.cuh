@@ -42,7 +42,6 @@ struct RenderIO {
     int N, S;
     int rays_per_tile;     // tensor-core kernel: chosen by its launcher
     float* rgb; float* depth; float* weights; float* alpha; float* input_feat;
-    long long* trace;      // debug timeline (mvsn_debug_set_trace), null in normal operation
     // multi-GPU frame sink (mvsn_render_rays_to_peers): every finished pixel is stored as one 16-byte
     // (r, g, b, depth) texel into EVERY rank's copy of the assembled frame, straight from the compositing
     // epilogue over NVLink peer mappings -- the frame is complete on all ranks when the kernels are, with no
@@ -80,8 +79,6 @@ int launch_adam_tensors(float* const* p, const float* const* g, float* const* m,
                         float lr, float beta1, float beta2, float eps, int step, cudaStream_t stream);
 int launch_adam_volume(float* p, float* g_dhwc, float* m, float* v, long long nvox, int planar, float lr, float beta1,
                        float beta2, float eps, int step, cudaStream_t stream);
-size_t mlp_tc2_packed_bytes();
-int pack_mlp_tc2(const float* const* w, void* packed, cudaStream_t stream);
 
 // cam = R p + t ; pix = K cam ; (u, v) = pix.xy / pix.z / (W-1, H-1)     utils.py:120-127
 template <bool PRECISE>
@@ -127,27 +124,73 @@ __device__ __forceinline__ void ndc_of_point(const SceneDev& sc, const Cams& cam
     nx = u; ny = v;
 }
 
+// ray-march depth at step t in [0, 1] (data/ray_utils.py:177-180), rounded as the reference's fp32 ops round
+__device__ __forceinline__ float ray_z(float near, float far, float t, int lindisp) {
+    if (!lindisp) return __fadd_rn(__fmul_rn(near, 1.f - t), __fmul_rn(far, t));
+    return __fdiv_rn(1.f, __fadd_rn(__fmul_rn(__fdiv_rn(1.f, near), 1.f - t), __fmul_rn(__fdiv_rn(1.f, far), t)));
+}
+
+// ray-march point (px, py, pz), ray direction (dx, dy, dz), NDC (nx, ny, nz) and depth z of sample s_idx of ray `ray`:
+// marched from io.rays / io.t_steps (FAST) or read from the caller's per-sample arrays (si = ray * S + s_idx)
+template <bool FAST, bool PRECISE>
+__device__ __forceinline__ void sample_point(const SceneDev& sc, const Cams& cams, const RenderIO& io, int ray, int s_idx,
+                                             size_t si, float& px, float& py, float& pz, float& dx, float& dy, float& dz,
+                                             float& nx, float& ny, float& nz, float& z) {
+    if (FAST) {
+        const float4* rp = reinterpret_cast<const float4*>(io.rays + (size_t)ray * 8);
+        float4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
+        dx = r0.w; dy = r1.x; dz = r1.y;
+        z = ray_z(r1.z, r1.w, __ldg(io.t_steps + s_idx), io.rg.lindisp);
+        px = __fadd_rn(r0.x, __fmul_rn(dx, z));
+        py = __fadd_rn(r0.y, __fmul_rn(dy, z));
+        pz = __fadd_rn(r0.z, __fmul_rn(dz, z));
+        ndc_of_point<PRECISE>(sc, cams, io.rg, px, py, pz, nx, ny, nz);
+    } else {
+        px = __ldg(io.pts + si * 3); py = __ldg(io.pts + si * 3 + 1); pz = __ldg(io.pts + si * 3 + 2);
+        nx = __ldg(io.ndc + si * 3); ny = __ldg(io.ndc + si * 3 + 1); nz = __ldg(io.ndc + si * 3 + 2);
+        z = io.z[si];                                   // plain load: removed where z is unused
+        dx = __ldg(io.dirs + (size_t)ray * 3); dy = __ldg(io.dirs + (size_t)ray * 3 + 1);
+        dz = __ldg(io.dirs + (size_t)ray * 3 + 2);
+    }
+}
+
+// Trilinear footprint of an NDC point in the volume (utils.py:357-383, align_corners=True): the corner origin and the
+// per-axis corner weights, with no masking.  Corner c = (x0 + (c & 1), y0 + ((c >> 1) & 1), z0 + (c >> 2)) has weight
+// wx[c & 1] * wy[(c >> 1) & 1] * wz[c >> 2]; corners outside the volume are the caller's to handle.
+struct Trilinear {
+    int x0, y0, z0;
+    float wx[2], wy[2], wz[2];
+};
+__device__ __forceinline__ Trilinear trilinear_corners(const SceneDev& sc, float nx, float ny, float nz) {
+    const int W = sc.Wp, H = sc.Hp, D = sc.D;
+    const float ix = ((nx * 2.f - 1.f + 1.f) * 0.5f) * (float)(W - 1);
+    const float iy = ((ny * 2.f - 1.f + 1.f) * 0.5f) * (float)(H - 1);
+    const float iz = ((nz * 2.f - 1.f + 1.f) * 0.5f) * (float)(D - 1);
+    const float x0f = floorf(ix), y0f = floorf(iy), z0f = floorf(iz);
+    Trilinear t;
+    t.wx[0] = (x0f + 1.f) - ix; t.wx[1] = ix - x0f;
+    t.wy[0] = (y0f + 1.f) - iy; t.wy[1] = iy - y0f;
+    t.wz[0] = (z0f + 1.f) - iz; t.wz[1] = iz - z0f;
+    // clamp before the int conversion so absurd coordinates cannot overflow
+    t.x0 = (int)fminf(fmaxf(x0f, -2.f), (float)W);
+    t.y0 = (int)fminf(fmaxf(y0f, -2.f), (float)H);
+    t.z0 = (int)fminf(fmaxf(z0f, -2.f), (float)D);
+    return t;
+}
+
 // utils.index_point_feature (utils.py:357-383): trilinear, zeros padding, align_corners=True.
 // All sixteen 16-byte loads are issued unconditionally (indices clamped, out-of-volume corners get
 // weight 0) so they are in flight together instead of one DRAM latency per corner.
 __device__ __forceinline__ void sample_volume(const SceneDev& sc, float nx, float ny, float nz, float* out8) {
     const int W = sc.Wp, H = sc.Hp, D = sc.D;
-    float ix = ((nx * 2.f - 1.f + 1.f) * 0.5f) * (float)(W - 1);
-    float iy = ((ny * 2.f - 1.f + 1.f) * 0.5f) * (float)(H - 1);
-    float iz = ((nz * 2.f - 1.f + 1.f) * 0.5f) * (float)(D - 1);
-    float x0f = floorf(ix), y0f = floorf(iy), z0f = floorf(iz);
-    float wx[2] = {(x0f + 1.f) - ix, ix - x0f}, wy[2] = {(y0f + 1.f) - iy, iy - y0f}, wz[2] = {(z0f + 1.f) - iz, iz - z0f};
-    // clamp before the int conversion so absurd coordinates cannot overflow
-    const int x0 = (int)fminf(fmaxf(x0f, -2.f), (float)W);
-    const int y0 = (int)fminf(fmaxf(y0f, -2.f), (float)H);
-    const int z0 = (int)fminf(fmaxf(z0f, -2.f), (float)D);
+    Trilinear t = trilinear_corners(sc, nx, ny, nz);
     int xo[2], yo[2], zo[2];
 #pragma unroll
     for (int d = 0; d < 2; ++d) {
-        const int x = x0 + d, y = y0 + d, z = z0 + d;
-        if ((unsigned)x >= (unsigned)W) wx[d] = 0.f;       // zeros padding: the tap contributes nothing
-        if ((unsigned)y >= (unsigned)H) wy[d] = 0.f;
-        if ((unsigned)z >= (unsigned)D) wz[d] = 0.f;
+        const int x = t.x0 + d, y = t.y0 + d, z = t.z0 + d;
+        if ((unsigned)x >= (unsigned)W) t.wx[d] = 0.f;     // zeros padding: the tap contributes nothing
+        if ((unsigned)y >= (unsigned)H) t.wy[d] = 0.f;
+        if ((unsigned)z >= (unsigned)D) t.wz[d] = 0.f;
         xo[d] = min(max(x, 0), W - 1); yo[d] = min(max(y, 0), H - 1); zo[d] = min(max(z, 0), D - 1);
     }
     float4 va[8], vb[8];
@@ -161,7 +204,7 @@ __device__ __forceinline__ void sample_volume(const SceneDev& sc, float nx, floa
     for (int c = 0; c < 8; ++c) out8[c] = 0.f;
 #pragma unroll
     for (int c = 0; c < 8; ++c) {                          // accumulation order as aten: x fastest, then y, then z
-        const float wgt = wx[c & 1] * wy[(c >> 1) & 1] * wz[c >> 2];
+        const float wgt = t.wx[c & 1] * t.wy[(c >> 1) & 1] * t.wz[c >> 2];
         out8[0] = fmaf(va[c].x, wgt, out8[0]); out8[1] = fmaf(va[c].y, wgt, out8[1]);
         out8[2] = fmaf(va[c].z, wgt, out8[2]); out8[3] = fmaf(va[c].w, wgt, out8[3]);
         out8[4] = fmaf(vb[c].x, wgt, out8[4]); out8[5] = fmaf(vb[c].y, wgt, out8[5]);

@@ -194,32 +194,6 @@ __device__ __forceinline__ void gemm_rs(float (&d)[N / 2], const uint32_t* ah, c
     }
 }
 
-// ray-march point (px, py, pz), ray direction (dx, dy, dz) and NDC (nx, ny, nz) of sample s_idx of ray `ray`
-template <bool FAST, bool PRECISE>
-__device__ __forceinline__ void sample_point(const SceneDev& sc, const Cams& cams, const RenderIO& io, int ray, int s_idx,
-                                             size_t si, float& px, float& py, float& pz, float& dx, float& dy, float& dz,
-                                             float& nx, float& ny, float& nz) {
-    if (FAST) {
-        const float4* rp = reinterpret_cast<const float4*>(io.rays + (size_t)ray * 8);
-        float4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
-        dx = r0.w; dy = r1.x; dz = r1.y;
-        const float near = r1.z, far = r1.w, tt = __ldg(io.t_steps + s_idx);
-        float zv;
-        if (!io.rg.lindisp) zv = __fadd_rn(__fmul_rn(near, 1.f - tt), __fmul_rn(far, tt));
-        else zv = __fdiv_rn(1.f, __fadd_rn(__fmul_rn(__fdiv_rn(1.f, near), 1.f - tt),
-                                           __fmul_rn(__fdiv_rn(1.f, far), tt)));
-        px = __fadd_rn(r0.x, __fmul_rn(dx, zv));
-        py = __fadd_rn(r0.y, __fmul_rn(dy, zv));
-        pz = __fadd_rn(r0.z, __fmul_rn(dz, zv));
-        ndc_of_point<PRECISE>(sc, cams, io.rg, px, py, pz, nx, ny, nz);
-    } else {
-        px = __ldg(io.pts + si * 3); py = __ldg(io.pts + si * 3 + 1); pz = __ldg(io.pts + si * 3 + 2);
-        nx = __ldg(io.ndc + si * 3); ny = __ldg(io.ndc + si * 3 + 1); nz = __ldg(io.ndc + si * 3 + 2);
-        dx = __ldg(io.dirs + (size_t)ray * 3); dy = __ldg(io.dirs + (size_t)ray * 3 + 1);
-        dz = __ldg(io.dirs + (size_t)ray * 3 + 2);
-    }
-}
-
 // Tile geometry (identical in every role).  A tile is RT rays x SP = 64/RT consecutive samples: row = sub * RT +
 // ray_in, so neighbouring rows are adjacent rays at the SAME sample index -- their volume / image taps fall in the
 // same few cache lines.  Ray and sample of row `row` of tile `tile` of ray group `grp`:
@@ -321,8 +295,8 @@ __device__ __forceinline__ void front_end(const SceneDev& sc, const Cams& cams, 
     const int row = t & (wg::ROWS - 1), part = t >> 6;
     const TileRow r(io, grp, tile, row);
     float nx = 0.f, ny = 0.f, nz = 0.f;
-    float px = 0.f, py = 0.f, pz = 0.f, dx = 0.f, dy = 0.f, dz = 1.f;
-    if (r.valid) sample_point<FAST, SPLIT>(sc, cams, io, r.ray, r.s_idx, r.si, px, py, pz, dx, dy, dz, nx, ny, nz);
+    float px = 0.f, py = 0.f, pz = 0.f, dx = 0.f, dy = 0.f, dz = 1.f, z;      // z: the compositing recomputes it
+    if (r.valid) sample_point<FAST, SPLIT>(sc, cams, io, r.ray, r.s_idx, r.si, px, py, pz, dx, dy, dz, nx, ny, nz, z);
     const float nd[3] = {nx, ny, nz};
     if (part == 0) {
         if (!SPLIT) store_volume_dir<SPLIT>(sc, cams, io, r, nd, dx, dy, dz, misc, row);
@@ -617,13 +591,8 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                     if (sj >= S) break;
                     const float4 v = reinterpret_cast<const float4*>(xch)[sub * RT + t];
                     float z;
-                    if (FAST) {
-                        const float tt = __ldg(io.t_steps + sj);
-                        if (!io.rg.lindisp) z = __fadd_rn(__fmul_rn(znear, 1.f - tt), __fmul_rn(zfar, tt));
-                        else z = __fdiv_rn(1.f, __fadd_rn(__fmul_rn(__fdiv_rn(1.f, znear), 1.f - tt), __fmul_rn(__fdiv_rn(1.f, zfar), tt)));
-                    } else {
-                        z = __ldg(io.z + (size_t)cray * S + sj);
-                    }
+                    if (FAST) z = ray_z(znear, zfar, __ldg(io.t_steps + sj), io.rg.lindisp);
+                    else      z = __ldg(io.z + (size_t)cray * S + sj);
                     const float wgt = v.x * cT;
                     if (io.alpha) io.alpha[(size_t)cray * S + sj] = v.x;
                     if (io.weights) io.weights[(size_t)cray * S + sj] = wgt;

@@ -24,7 +24,7 @@ EXPORTS = [
     "mvsn_render_samples", "mvsn_render_rays", "mvsn_cost_volume_workspace_bytes",
     "mvsn_build_cost_volume", "mvsn_costreg_workspace_bytes", "mvsn_costreg_forward",
     "mvsn_featurenet_workspace_bytes", "mvsn_featurenet_forward",
-    "mvsn_selftest_umma", "mvsn_debug_set_trace",
+    "mvsn_selftest_umma",
     "mvsn_peer_buffer_create", "mvsn_peer_buffer_open", "mvsn_peer_buffer_close", "mvsn_peer_buffer_destroy",
     "mvsn_render_rays_to_peers", "mvsn_make_rays",
     "mvsn_featurenet_forward_bn", "mvsn_costreg_forward_bn",
@@ -106,8 +106,6 @@ def load() -> C.CDLL:
     lib.mvsn_featurenet_forward_bn.argtypes = [C.POINTER(vp), C.POINTER(vp), ip, fp, vp, ip, ip, ip, vp, vp, C.c_size_t, vp]
     lib.mvsn_make_rays.argtypes = [vp, vp, fp, fp, ip, vp, vp]
     lib.mvsn_make_rays.restype = ip
-    lib.mvsn_debug_set_trace.argtypes = [vp]
-    lib.mvsn_debug_set_trace.restype = None
     lib.mvsn_selftest_umma.argtypes = [vp, vp, vp, ip, ip, vp, vp]
     for name in ("mvsn_selftest_umma", "mvsn_mlp_pack", "mvsn_pack_images", "mvsn_volume_to_channels_last",
                  "mvsn_volume_from_channels_last", "mvsn_render_samples", "mvsn_render_rays",

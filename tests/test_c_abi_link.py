@@ -20,7 +20,7 @@ int main(void) {
     struct mvsn_ray_params rp;
     memset(&sc, 0, sizeof sc);
     memset(&rp, 0, sizeof rp);
-    if (mvsn_abi_version() != 1) return 1;
+    if (mvsn_abi_version() != 2) return 1;
     if (mvsn_mlp_packed_bytes(MVSN_MLP_FP32) == 0 || mvsn_mlp_packed_bytes(MVSN_MLP_TC_HALF) == 0 ||
         mvsn_mlp_packed_bytes(MVSN_MLP_TC_SPLIT) == 0 || mvsn_mlp_packed_bytes(77) != 0) return 2;
     if (mvsn_costreg_workspace_bytes(128, 176, 208) == 0 || mvsn_featurenet_workspace_bytes(3, 512, 640) == 0 ||
@@ -37,7 +37,7 @@ int main(void) {
 
 
 @pytest.mark.skipif(shutil.which("gcc") is None, reason="no C compiler")
-def test_header_is_c_and_library_links_from_c(tmp_path):
+def test_header_is_c_and_abi2_library_links_from_c(tmp_path):
     lib_path = build.build_library()
     src = tmp_path / "abi_check.c"
     src.write_text(C_SRC)
@@ -49,4 +49,4 @@ def test_header_is_c_and_library_links_from_c(tmp_path):
     assert r.returncode == 0, r.stderr
     r = subprocess.run([str(exe)], capture_output=True, text=True)
     assert r.returncode == 0, (r.returncode, r.stdout, r.stderr)
-    assert "abi 1 ok" in r.stdout
+    assert "abi 2 ok" in r.stdout

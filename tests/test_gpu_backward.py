@@ -82,6 +82,28 @@ def test_backward_kernel_vs_oracle_autograd_all_outputs(scene, weights, S, n, wh
     _assert_close(g_vol.permute(3, 0, 1, 2).unsqueeze(0).cpu(), vt.grad, 2e-4, "volume")
 
 
+@pytest.mark.parametrize("S,n,white", [(32, 130, True), (48, 21, False), (128, 37, False), (128, 300, True)])
+def test_backward_recompute_renders_what_the_fp32_kernel_renders(scene, S, n, white):
+    """The backward kernel's forward recompute and mlp_mode=MLP_FP32 rendering run the same fp32 forward tile, so the
+    rgb the backward reports is bit-identical to the render kernel's on the same samples.  Depth is composed with
+    different rounding in the two kernels (fmaf vs multiply-then-add), so it agrees to 1e-6 only."""
+    sc, vol_ref = scene
+    rays, pts, ndc, z = _samples(sc, n, S, seed=S + n, perturb=1.0)
+    fn = backend.MVSNeRF().to(DEV)
+    backend.load_weights_npz(fn, None, WPATH)
+    d = sc.to(DEV)
+    vol = vol_ref.to(DEV)
+    pts, ndc, z, rd = pts.to(DEV), ndc.to(DEV), z.to(DEV), rays[:, 3:6].to(DEV)
+    _, _, rgb_b, depth_b = backend.render_backward(d.pose_source, pts, ndc, z, rd, vol, d.imgs_raw, fn, white,
+                                                   grads={"rgb": torch.ones(n, 3, device=DEV)}, want_forward=True)
+    with torch.no_grad():
+        rgb_f, _, _, depth_f, _, _ = backend.rendering(Args(), d.pose_source, pts, ndc, z, None, rd, volume_feature=vol,
+                                                       imgs=d.imgs_raw, network_fn=fn, white_bkgd=white,
+                                                       mlp_mode=lib.MLP_FP32)
+    assert torch.equal(rgb_b, rgb_f), (rgb_b - rgb_f).abs().max().item()
+    assert (depth_b - depth_f).abs().max().item() <= 1e-6
+
+
 @pytest.mark.parametrize("tag,white", [("s32", False), ("s128w", True)])
 def test_backward_kernel_vs_reference_gradient_fixture(golden_grad, golden_tiny, tag, white):
     """The fused-loss launch (img2mse formed in the kernel) against gradients the unmodified reference's autograd

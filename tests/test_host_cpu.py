@@ -17,7 +17,7 @@ def built():
     return build.build_library()
 
 
-def test_library_exports_every_declared_symbol(built):
+def test_abi2_library_exports_every_declared_symbol(built):
     header = open(os.path.join(ROOT, "include", "mvsnerf_b200.h")).read()
     declared = sorted(set(re.findall(r"\b(mvsn_[a-z0-9_]+)\s*\(", header)))
     assert declared == sorted(lib.EXPORTS)
@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol(built):
     for name in declared:
         assert hasattr(dll, name), name
     L = lib.load()
-    assert L.mvsn_abi_version() == 1
+    assert L.mvsn_abi_version() == 2
     assert L.mvsn_mlp_packed_bytes(lib.MLP_FP32) > 126788 * 4
     assert L.mvsn_costreg_workspace_bytes(128, 176, 208) > 400e6
     assert L.mvsn_cost_volume_workspace_bytes(3, 128, 160) == 3 * 128 * 160 * (4 + 32) * 4
