@@ -173,6 +173,16 @@ int mvsn_render_backward(const mvsn_render_scene* scene, const float* const* mlp
                          const float* rays_pts, const float* rays_ndc, const float* z_vals, const float* rays_dir,
                          int N, int S, const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc,
                          void* workspace, size_t workspace_bytes, void* stream);
+/* mvsn_render_backward_tc: the same call, arguments and outputs as mvsn_render_backward (scene->mlp_packed is still
+ * the MVSN_MLP_FP32 image, used by the forward recompute; N_samples <= 128, otherwise MVSN_EUNSUPPORTED), with the
+ * MLP dgrad / wgrad GEMMs on tensor cores: dpre, layer inputs and weights rounded to fp16 (each tile with an exact
+ * power-of-two scale), fp32 accumulation.  rgb_out / depth_out are bit-identical to mvsn_render_backward's, and so is
+ * each ray's loss term (loss_out sums them with float atomics); gradients agree with it to ~1e-3 of their max |g|.  Workspace: mvsn_render_backward_tc_workspace_bytes(N, S). */
+size_t mvsn_render_backward_tc_workspace_bytes(int N, int S);
+int mvsn_render_backward_tc(const mvsn_render_scene* scene, const float* const* mlp_w,
+                            const float* rays_pts, const float* rays_ndc, const float* z_vals, const float* rays_dir,
+                            int N, int S, const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc,
+                            void* workspace, size_t workspace_bytes, void* stream);
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
                    const int* numel_host, int count, float lr, float beta1, float beta2, float eps, int step,
                    void* stream);

@@ -466,12 +466,15 @@ def rendering(args, pose_ref, rays_pts, rays_ndc, depth_candidates, rays_o, rays
     Extra keyword arguments the reference's callers pass (perturb, N_importance, network_fine,
     use_viewdirs, raw_noise_std, NDC_local) are accepted and ignored, as the reference does.
     `mlp_mode=` selects the GEMM arithmetic (default: DEFAULT_MLP_MODE, the fp32-grade tensor mode); `want_aux=False` skips the three
-    per-sample outputs (they are returned as None)."""
+    per-sample outputs (they are returned as None).  Under autograd, `grad_mode=` selects the arithmetic of the backward's
+    GEMMs (see render_backward; default MLP_FP32)."""
     if pose_ref is None or img_feat is not None or getattr(args, "use_color_volume", False):
         raise RuntimeError("rendering: only the pose_ref / image-gather branch of the reference is implemented "
                            "(use_color_volume=False, img_feat=None) -- the branch every shipped config uses")
     mode = kwargs.pop("mlp_mode", DEFAULT_MLP_MODE)
     want_aux = kwargs.pop("want_aux", True)
+    grad_mode = kwargs.pop("grad_mode", _lib.MLP_FP32)
+    _check_grad_mode(grad_mode)
     N, S = rays_pts.shape[:2]
     z = depth_candidates.expand(N, S) if depth_candidates.shape != (N, S) else depth_candidates
     vol_t = volume_feature.feat_volume if isinstance(volume_feature, nn.Module) else volume_feature
@@ -481,7 +484,7 @@ def rendering(args, pose_ref, rays_pts, rays_ndc, depth_candidates, rays_o, rays
         params = network_fn.ordered_params()
         rgb, feat, weights, depth, alpha = _RenderSamplesFn.apply(
             rays_pts, rays_ndc, z, rays_dir, vol_t, imgs, pose_ref["w2cs"], pose_ref["intrinsics"],
-            bool(white_bkgd), mode, network_fn, volume_feature, *params)
+            bool(white_bkgd), mode, network_fn, volume_feature, grad_mode, *params)
         return rgb, feat, weights, depth, alpha, {}
     rgb, feat, weights, depth, alpha = _render_samples_kernel(
         pose_ref, rays_pts, rays_ndc, z, rays_dir, volume_feature, imgs, network_fn, white_bkgd, mode, want_aux)
@@ -550,17 +553,19 @@ class _RenderSamplesFn(torch.autograd.Function):
     forward: the fused CUDA kernel, exactly as in inference (no graph, nothing per-sample kept).
     backward: gradients w.r.t. the 22 MLP tensors and the encoding volume.  With N_samples <= 128 (and
     BACKWARD_IMPL == "kernel") they come from the backward kernel (csrc/render_bwd.cu: forward recompute on the
-    fp32 render kernel's own forward tile, MLP dgrad/wgrad, trilinear scatter into the volume gradient).  Otherwise
+    fp32 render kernel's own forward tile, MLP dgrad/wgrad in the arithmetic `grad_mode` selects, trilinear scatter
+    into the volume gradient).  Otherwise
     the chunk is re-evaluated with PyTorch ops under autograd (_render_samples_torch); activation memory then
     exists only during backward."""
 
     @staticmethod
     def forward(ctx, pts, ndc, z, rays_dir, vol, imgs, w2cs, intrinsics, white_bkgd, mode, network_fn, volume_feature,
-                *params):
+                grad_mode, *params):
         pose = {"w2cs": w2cs, "intrinsics": intrinsics}
         out = _render_samples_kernel(pose, pts, ndc, z, rays_dir, volume_feature, imgs, network_fn, white_bkgd, mode)
         ctx.save_for_backward(pts, ndc, z, rays_dir, vol, imgs, w2cs, intrinsics, *params)
         ctx.white_bkgd, ctx.network_fn, ctx.volume_feature = white_bkgd, network_fn, volume_feature
+        ctx.grad_mode = grad_mode
         return out
 
     @staticmethod
@@ -573,14 +578,14 @@ class _RenderSamplesFn(torch.autograd.Function):
             grads = {"rgb": g_rgb, "depth": g_depth, "weights": g_weights, "alpha": g_alpha, "input_feat": g_feat}
             g_params, dvol, _, _ = render_backward(
                 {"w2cs": w2cs, "intrinsics": intrinsics}, pts, ndc, z, rays_dir, ctx.volume_feature, imgs, ctx.network_fn,
-                ctx.white_bkgd, grads=grads, want_volume_grad=need_vol)
+                ctx.white_bkgd, grads=grads, want_volume_grad=need_vol, grad_mode=ctx.grad_mode)
             g_vol = dvol.permute(3, 0, 1, 2).unsqueeze(0) if need_vol else None
-            g_params = [g if need else None for g, need in zip(g_params, ctx.needs_input_grad[12:])]
-            return (None, None, None, None, g_vol, None, None, None, None, None, None, None, *g_params)
+            g_params = [g if need else None for g, need in zip(g_params, ctx.needs_input_grad[13:])]
+            return (None, None, None, None, g_vol, None, None, None, None, None, None, None, None, *g_params)
         with torch.enable_grad():
             vol_g = vol.detach().requires_grad_(ctx.needs_input_grad[4])
             # evaluate through a functional copy of the module so the user's parameters are not touched
-            leaves = [p.detach().requires_grad_(need) for p, need in zip(params, ctx.needs_input_grad[12:])]
+            leaves = [p.detach().requires_grad_(need) for p, need in zip(params, ctx.needs_input_grad[13:])]
             names = [n for n, _ in _ordered_named_params(ctx.network_fn)]
             nerf = lambda x: torch.func.functional_call(ctx.network_fn, dict(zip(names, leaves)), (x,))
             outs = _render_samples_torch(pts.detach(), ndc.detach(), z.detach(), rays_dir.detach(), vol_g, imgs.detach(),
@@ -592,7 +597,7 @@ class _RenderSamplesFn(torch.autograd.Function):
         it = iter(grads)
         g_vol = next(it) if vol_g.requires_grad and grads else None
         g_params = [next(it) if (leaf.requires_grad and grads) else None for leaf in leaves]
-        return (None, None, None, None, g_vol, None, None, None, None, None, None, None, *g_params)
+        return (None, None, None, None, g_vol, None, None, None, None, None, None, None, None, *g_params)
 
 
 # "kernel": csrc/render_bwd.cu (N_samples <= 128); "torch": the PyTorch-recompute backward above (kept as the
@@ -601,9 +606,18 @@ BACKWARD_IMPL = "kernel"
 _bwd_workspace = {}
 
 
-def _backward_workspace(dev, N, S):
+def _check_grad_mode(grad_mode):
+    if grad_mode not in (_lib.MLP_FP32, _lib.MLP_TC_HALF):
+        raise RuntimeError(f"grad_mode {grad_mode!r}: the backward's GEMMs run in MLP_FP32 (FFMA) or MLP_TC_HALF "
+                           "(wgmma, fp16 operands with per-tile power-of-two scales, fp32 accumulation)")
+
+
+def _backward_workspace(dev, N, S, grad_mode=_lib.MLP_FP32):
     lib = _lib.load()
-    need = lib.mvsn_render_backward_workspace_bytes(int(N), int(S))
+    if grad_mode == _lib.MLP_TC_HALF:
+        need = lib.mvsn_render_backward_tc_workspace_bytes(int(N), int(S))
+    else:
+        need = lib.mvsn_render_backward_workspace_bytes(int(N), int(S))
     if need == 0:
         raise RuntimeError(f"render backward: unsupported shape N={N}, N_samples={S} (N_samples <= 128)")
     ws = _bwd_workspace.get(dev)
@@ -615,12 +629,15 @@ def _backward_workspace(dev, N, S):
 
 def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_feature, imgs, network_fn, white_bkgd=False,
                     grads=None, target_rgb=None, n_total=None, want_volume_grad=True, grad_volume=None, grad_mlp=None,
-                    want_forward=False, loss_out=None):
-    """One mvsn_render_backward launch.  Either `grads` (dict with 'rgb' and optionally 'depth', 'weights', 'alpha',
+                    want_forward=False, loss_out=None, grad_mode=_lib.MLP_FP32):
+    """One mvsn_render_backward launch (grad_mode=MLP_FP32: fp32 FFMA GEMMs) or mvsn_render_backward_tc launch
+    (grad_mode=MLP_TC_HALF: the dgrad / wgrad GEMMs on tensor cores with fp16 operands, fp32 accumulation; the forward
+    recompute, and so rgb / depth / the loss, are the same fp32 tile and bit-identical).  Either `grads` (dict with 'rgb' and optionally 'depth', 'weights', 'alpha',
     'input_feat': d loss / d output of `rendering`) or `target_rgb` [N,3] (img2mse formed in the kernel, normalised by
     3 * n_total).  Returns (grad_mlp[22] in ordered_params() order, grad_volume [D,Hp,Wp,8] channels-last or None,
     rgb [N,3] or None, depth [N] or None).  `grad_volume` (accumulated into) and `grad_mlp` (overwritten) may be passed
     to reuse buffers."""
+    _check_grad_mode(grad_mode)
     lib = _lib.load()
     N, S = rays_pts.shape[:2]
     dev = rays_pts.device
@@ -665,12 +682,14 @@ def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_featu
         g.rgb_out, g.depth_out = rgb.data_ptr(), depth.data_ptr()
     if loss_out is not None:
         g.loss_out = loss_out.data_ptr()
-    ws, ws_bytes = _backward_workspace(dev, N, S)
+    ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode)
+    entry, name = ((lib.mvsn_render_backward_tc, "mvsn_render_backward_tc") if grad_mode == _lib.MLP_TC_HALF
+                   else (lib.mvsn_render_backward, "mvsn_render_backward"))
     with torch.cuda.device(dev):
-        _lib.check(lib.mvsn_render_backward(C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z),
-                                            _lib.ptr(dirs), N, S, C.byref(g), _lib.ptr_array(grad_mlp),
-                                            _lib.ptr(grad_volume) if want_volume_grad else None, _lib.ptr(ws), ws_bytes,
-                                            _lib.stream_ptr()), "mvsn_render_backward")
+        _lib.check(entry(C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z),
+                         _lib.ptr(dirs), N, S, C.byref(g), _lib.ptr_array(grad_mlp),
+                         _lib.ptr(grad_volume) if want_volume_grad else None, _lib.ptr(ws), ws_bytes,
+                         _lib.stream_ptr()), name)
     del keep, held
     return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
 
@@ -683,9 +702,13 @@ class FineTuner:
         -> mvsn_adam_step (22 MLP tensors) -> mvsn_adam_step_volume (volume; also zeroes its gradient buffer)
 
     The parameters stay the caller's nn.Parameters (updated in place, version counters bumped), so checkpoints, the
-    render entry points and scene_io see them as after a torch.optim.Adam step with the same hyper-parameters."""
+    render entry points and scene_io see them as after a torch.optim.Adam step with the same hyper-parameters.
+    grad_mode=MLP_TC_HALF runs the backward's dgrad / wgrad GEMMs on tensor cores (see render_backward)."""
 
-    def __init__(self, network_fn, volume, imgs, pose_ref, lr=5e-4, betas=(0.9, 0.999), eps=1e-8, white_bkgd=False):
+    def __init__(self, network_fn, volume, imgs, pose_ref, lr=5e-4, betas=(0.9, 0.999), eps=1e-8, white_bkgd=False,
+                 grad_mode=_lib.MLP_FP32):
+        _check_grad_mode(grad_mode)
+        self.grad_mode = grad_mode
         self.network_fn, self.volume, self.imgs, self.pose_ref = network_fn, volume, imgs, pose_ref
         self.lr, self.betas, self.eps, self.white_bkgd = float(lr), (float(betas[0]), float(betas[1])), float(eps), bool(white_bkgd)
         self.step_count = 0
@@ -722,7 +745,7 @@ class FineTuner:
         _, _, rgb, depth = render_backward(self.pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, self.volume, self.imgs,
                                            self.network_fn, self.white_bkgd, target_rgb=target_rgb, want_volume_grad=True,
                                            grad_volume=self.vol_g, grad_mlp=self.g, want_forward=want_forward,
-                                           loss_out=self.loss)
+                                           loss_out=self.loss, grad_mode=self.grad_mode)
         dev = self.params[0].device
         fv = self.volume.feat_volume
         with torch.cuda.device(dev):
@@ -779,10 +802,11 @@ def get_ndc_coordinate(w2c_ref, intrinsic_ref, point_samples, inv_scale, near=2,
     return q.view(n, s, 3)
 
 
-def finetune_step_timing(dev, weights_npz, steps=20, warmup=5, batch=1024, n_samples=128):
+def finetune_step_timing(dev, weights_npz, steps=20, warmup=5, batch=1024, n_samples=128, grad_mode=_lib.MLP_FP32):
     """bench.py's BASELINE-config-3 entry: fine-tuning steps on a Blender-shaped scene (800x800, pad 0, white_bkgd,
     near_far [2, 6]; encoding volume 8x128x200x200), 1024 rays x 128 samples per step, perturb = 1 -- the fused
-    FineTuner step and, beside it, the same step through `rendering` under autograd + torch.optim.Adam."""
+    FineTuner step and, beside it, the same step through `rendering` under autograd + torch.optim.Adam.  `grad_mode`
+    selects the arithmetic of the backward's GEMMs in both."""
     from . import synthetic
     fn, mvs = MVSNeRF().to(dev), MVSNet().to(dev).train()
     load_weights_npz(fn, mvs, weights_npz)
@@ -818,7 +842,7 @@ def finetune_step_timing(dev, weights_npz, steps=20, warmup=5, batch=1024, n_sam
 
     out = {"rays": batch, "n_samples": n_samples, "volume": list(vol.shape), "white_bkgd": True}
     volume = RefVolume(vol.detach().clone()).to(dev)
-    tuner = FineTuner(fn, volume, d.imgs_raw, d.pose_source, lr=5e-4, white_bkgd=True)
+    tuner = FineTuner(fn, volume, d.imgs_raw, d.pose_source, lr=5e-4, white_bkgd=True, grad_mode=grad_mode)
     losses = []
     out["fused_ms"] = timed(lambda xyz, ndc, z, rd, tgt: losses.append(tuner.step(xyz, ndc, z, rd, tgt)[0].clone()))
     out["fused_loss_first_last"] = [float(losses[0]), float(losses[-1])]
@@ -832,7 +856,7 @@ def finetune_step_timing(dev, weights_npz, steps=20, warmup=5, batch=1024, n_sam
 
     def autograd_step(xyz, ndc, z, rd, tgt):
         rgb = rendering(args, d.pose_source, xyz, ndc, z, None, rd, volume2, d.imgs_raw, network_fn=fn2, white_bkgd=True,
-                        want_aux=True)[0]
+                        want_aux=True, grad_mode=grad_mode)[0]
         loss = torch.mean((rgb - tgt) ** 2)
         opt.zero_grad(set_to_none=True)
         loss.backward()

@@ -308,12 +308,12 @@ int mvsn_make_rays(const float* directions, const float* c2w, float near, float 
 
 // ---- fine-tuning step ------------------------------------------------------------------------------------
 size_t mvsn_render_backward_workspace_bytes(int N, int S) { return render_backward_workspace_bytes(N, S); }
+size_t mvsn_render_backward_tc_workspace_bytes(int N, int S) { return render_backward_tc_workspace_bytes(N, S); }
 
-int mvsn_render_backward(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
-                         const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
-                         const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
-                         size_t workspace_bytes, void* stream) {
-    MVSN_RANGE("mvsn_render_backward");
+static int render_backward_entry(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                                 const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                                 const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc,
+                                 void* workspace, size_t workspace_bytes, void* stream, bool tc) {
     SceneDev sc;
     int rc = make_scene(scene, sc);
     if (rc) return rc;
@@ -333,7 +333,25 @@ int mvsn_render_backward(const mvsn_render_scene* scene, const float* const* mlp
     return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
                                   g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
                                   grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
-                                  (cudaStream_t)stream);
+                                  (cudaStream_t)stream, tc);
+}
+
+int mvsn_render_backward(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                         const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                         const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward");
+    return render_backward_entry(scene, mlp_w, rays_pts, rays_ndc, z_vals, rays_dir, N, S, g, grad_mlp, grad_volume_dhwc,
+                                 workspace, workspace_bytes, stream, false);
+}
+
+int mvsn_render_backward_tc(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                            const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                            const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward_tc");
+    return render_backward_entry(scene, mlp_w, rays_pts, rays_ndc, z_vals, rays_dir, N, S, g, grad_mlp, grad_volume_dhwc,
+                                 workspace, workspace_bytes, stream, true);
 }
 
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,

@@ -24,7 +24,11 @@
 //     the only atomics are the volume scatter (red.global.add.v4.f32, 16 per sample).
 // Gradient inputs: d rgb (required, or a target image for the fused MSE loss), d depth, d weights, d alpha,
 // d input_feat (optional) -- everything `rendering` returns is differentiable as in the reference.
+//
+// grad_mode MVSN_MLP_TC_HALF (mvsn_render_backward_tc) runs render_bwd_tc_kernel instead: the same tile with its
+// dgrad / wgrad GEMMs on wgmma with fp16 operands; its schedule and numerics are described above the kernel.
 #include "tile_fp32.cuh"
+#include "hopper.cuh"
 
 namespace mvsn {
 
@@ -155,6 +159,114 @@ constexpr int BWD_SMEM_FLOATS = TILE_SMEM_FLOATS + TILE_M * 18;
 constexpr size_t BWD_SMEM_BYTES = BWD_SMEM_FLOATS * sizeof(float);
 static_assert(TILE_M * PE_LD >= 64 * H_LD, "peT staging [64][H_LD] must fit in the positional-encoding region");
 
+// Compositing of a tile, forward and reverse scan, one thread per ray (renderer.py:65-92).  Writes rgb_out /
+// depth_out / the fused loss, s_T (transmittance in front of each sample) and s_g (d rgb_pre, d sigma_pre per row).
+// f_j = 1 - alpha_j + 1e-10, T_{j+1} = T_j f_j, w_j = alpha_j T_j.
+// d alpha_j = T_j (d w_j - B_j),  B_{j-1} = d w_j alpha_j + f_j B_j  (no division by f_j).
+__device__ __forceinline__ void composite_scan(const SceneDev& sc, const BwdIO& bw, const TileSmem& sm, float* s_T, float* s_g,
+                                               int grp, int R, int S, int N, int tid) {
+    if (tid < R) {
+        const int ray = grp * R + tid, first = tid * S;
+        if (ray < N) {
+            float cr = 0.f, cg = 0.f, cb = 0.f, dp = 0.f, ac = 0.f, T = 1.f;
+            for (int j = first; j < first + S; ++j) {
+                const float a = sm.rgb[j * 4 + 3], w = a * T;
+                s_T[j] = T;
+                cr = fmaf(w, sm.rgb[j * 4 + 0], cr); cg = fmaf(w, sm.rgb[j * 4 + 1], cg); cb = fmaf(w, sm.rgb[j * 4 + 2], cb);
+                dp = fmaf(w, sm.z[j], dp); ac += w;
+                T *= (1.f - a) + 1e-10f;
+            }
+            if (sc.white_bkgd) { const float bg = 1.f - ac; cr += bg; cg += bg; cb += bg; }
+            if (bw.rgb_out) { bw.rgb_out[(size_t)ray * 3] = cr; bw.rgb_out[(size_t)ray * 3 + 1] = cg; bw.rgb_out[(size_t)ray * 3 + 2] = cb; }
+            if (bw.depth_out) bw.depth_out[ray] = dp;
+            float g0, g1, g2;
+            if (bw.target) {                     // fused img2mse (utils.py: mean((rgb - target)^2))
+                const float e0 = cr - __ldg(bw.target + (size_t)ray * 3), e1 = cg - __ldg(bw.target + (size_t)ray * 3 + 1),
+                            e2 = cb - __ldg(bw.target + (size_t)ray * 3 + 2);
+                g0 = 2.f * e0 * bw.inv_count; g1 = 2.f * e1 * bw.inv_count; g2 = 2.f * e2 * bw.inv_count;
+                if (bw.loss) atomicAdd(bw.loss, (e0 * e0 + e1 * e1 + e2 * e2) * bw.inv_count);
+            } else {
+                g0 = __ldg(bw.g_rgb + (size_t)ray * 3); g1 = __ldg(bw.g_rgb + (size_t)ray * 3 + 1); g2 = __ldg(bw.g_rgb + (size_t)ray * 3 + 2);
+            }
+            const float gd = bw.g_depth ? __ldg(bw.g_depth + ray) : 0.f;
+            const float gbg = sc.white_bkgd ? (g0 + g1 + g2) : 0.f;
+            float B = 0.f;
+            for (int j = first + S - 1; j >= first; --j) {
+                const size_t sj = (size_t)ray * S + (j - first);
+                const float a = sm.rgb[j * 4 + 3], Tj = s_T[j], w = a * Tj;
+                const float c0 = sm.rgb[j * 4], c1 = sm.rgb[j * 4 + 1], c2 = sm.rgb[j * 4 + 2];
+                float dw = g0 * c0 + g1 * c1 + g2 * c2 + gd * sm.z[j] - gbg;
+                if (bw.g_weights) dw += __ldg(bw.g_weights + sj);
+                float da = Tj * (dw - B);
+                if (bw.g_alpha) da += __ldg(bw.g_alpha + sj);
+                B = fmaf(((1.f - a) + 1e-10f), B, dw * a);
+                s_g[j * 4 + 0] = w * g0 * c0 * (1.f - c0);
+                s_g[j * 4 + 1] = w * g1 * c1 * (1.f - c1);
+                s_g[j * 4 + 2] = w * g2 * c2 * (1.f - c2);
+                s_g[j * 4 + 3] = sm.sig[j] > 0.f ? da * (1.f - a) : 0.f;
+            }
+        } else {
+            for (int j = first; j < first + S; ++j) { s_g[j * 4] = s_g[j * 4 + 1] = s_g[j * 4 + 2] = s_g[j * 4 + 3] = 0.f; }
+        }
+    }
+    if (tid >= R * S && tid < TILE_M) { s_g[tid * 4] = s_g[tid * 4 + 1] = s_g[tid * 4 + 2] = s_g[tid * 4 + 3] = 0.f; }
+}
+
+// Element-wise stage of trunk layer l on the thread's fragment: acc = d h_{l+1}  ->  d g = acc * (h > 0) ;
+// d pre = d g * mod (left in acc) ; d mod += d g * pre, pre = h / mod (accumulated transposed in the scratch)
+__device__ __forceinline__ void trunk_elementwise(float (&acc)[8][8], float* scr, int l, int tid) {
+    const int ty = tid >> 4, tx = tid & 15;
+    const float* hT = scr + bwd::S_HT + l * 16384;
+    const float* mT = scr + bwd::S_MODT;
+#pragma unroll
+    for (int n = 0; n < 8; ++n) {
+        const int col = frag_col(tx, n);
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            const float4 h4 = *reinterpret_cast<const float4*>(hT + col * 128 + half * 64 + ty * 4);
+            const float4 m4 = *reinterpret_cast<const float4*>(mT + col * 128 + half * 64 + ty * 4);
+            const float hh[4] = {h4.x, h4.y, h4.z, h4.w}, mm[4] = {m4.x, m4.y, m4.z, m4.w};
+            float dm[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int r = half * 4 + i;
+                const bool on = hh[i] > 0.f;
+                const float dg = on ? acc[r][n] : 0.f;
+                acc[r][n] = dg * mm[i];
+                dm[i] = on ? dg * __fdiv_rn(hh[i], mm[i]) : 0.f;
+            }
+            float4* dmod = reinterpret_cast<float4*>(scr + bwd::S_DMOD + col * 128 + half * 64 + ty * 4);
+            float4 o = make_float4(dm[0], dm[1], dm[2], dm[3]);
+            if (l != 5) { const float4 p = *dmod; o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w; }
+            *dmod = o;
+        }
+    }
+}
+
+// Trilinear scatter of row `tid`'s 8 volume-feature gradients (s_df, plus d input_feat) into the channels-last volume
+// gradient: the transpose of utils.index_point_feature (utils.py:357-383), with the same corner weights.
+__device__ __forceinline__ void volume_scatter(const SceneDev& sc, const RenderIO& io, const BwdIO& bw, const float* s_df,
+                                               size_t si, int tid) {
+    float g8[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) g8[c] = s_df[tid * 8 + c];
+    if (bw.g_feat) {
+#pragma unroll
+        for (int c = 0; c < 8; ++c) g8[c] += __ldg(bw.g_feat + si * 20 + c);
+    }
+    const Trilinear t = trilinear_corners(sc, __ldg(io.ndc + si * 3), __ldg(io.ndc + si * 3 + 1), __ldg(io.ndc + si * 3 + 2));
+    const int W = sc.Wp, H = sc.Hp, D = sc.D;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        const int x = t.x0 + (c & 1), y = t.y0 + ((c >> 1) & 1), z = t.z0 + (c >> 2);
+        if ((unsigned)x >= (unsigned)W || (unsigned)y >= (unsigned)H || (unsigned)z >= (unsigned)D) continue;   // zeros padding
+        const float wgt = t.wx[c & 1] * t.wy[(c >> 1) & 1] * t.wz[c >> 2];
+        float4* p = reinterpret_cast<float4*>(bw.dvol + (((size_t)z * H + y) * W + x) * 8);
+        atomicAdd(p, make_float4(g8[0] * wgt, g8[1] * wgt, g8[2] * wgt, g8[3] * wgt));
+        atomicAdd(p + 1, make_float4(g8[4] * wgt, g8[5] * wgt, g8[6] * wgt, g8[7] * wgt));
+    }
+}
+
 __global__ void __launch_bounds__(256, 1)
 render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts) {
     extern __shared__ __align__(16) float smem[];
@@ -191,53 +303,7 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
         __syncthreads();
 
         // =============================== compositing: forward + reverse scan ===========================
-        // one thread per ray (renderer.py:65-92).  f_j = 1 - alpha_j + 1e-10, T_{j+1} = T_j f_j, w_j = alpha_j T_j.
-        // d alpha_j = T_j (d w_j - B_j),  B_{j-1} = d w_j alpha_j + f_j B_j  (no division by f_j).
-        if (tid < R) {
-            const int ray = grp * R + tid, first = tid * S;
-            if (ray < N) {
-                float cr = 0.f, cg = 0.f, cb = 0.f, dp = 0.f, ac = 0.f, T = 1.f;
-                for (int j = first; j < first + S; ++j) {
-                    const float a = sm.rgb[j * 4 + 3], w = a * T;
-                    s_T[j] = T;
-                    cr = fmaf(w, sm.rgb[j * 4 + 0], cr); cg = fmaf(w, sm.rgb[j * 4 + 1], cg); cb = fmaf(w, sm.rgb[j * 4 + 2], cb);
-                    dp = fmaf(w, sm.z[j], dp); ac += w;
-                    T *= (1.f - a) + 1e-10f;
-                }
-                if (sc.white_bkgd) { const float bg = 1.f - ac; cr += bg; cg += bg; cb += bg; }
-                if (bw.rgb_out) { bw.rgb_out[(size_t)ray * 3] = cr; bw.rgb_out[(size_t)ray * 3 + 1] = cg; bw.rgb_out[(size_t)ray * 3 + 2] = cb; }
-                if (bw.depth_out) bw.depth_out[ray] = dp;
-                float g0, g1, g2;
-                if (bw.target) {                     // fused img2mse (utils.py: mean((rgb - target)^2))
-                    const float e0 = cr - __ldg(bw.target + (size_t)ray * 3), e1 = cg - __ldg(bw.target + (size_t)ray * 3 + 1),
-                                e2 = cb - __ldg(bw.target + (size_t)ray * 3 + 2);
-                    g0 = 2.f * e0 * bw.inv_count; g1 = 2.f * e1 * bw.inv_count; g2 = 2.f * e2 * bw.inv_count;
-                    if (bw.loss) atomicAdd(bw.loss, (e0 * e0 + e1 * e1 + e2 * e2) * bw.inv_count);
-                } else {
-                    g0 = __ldg(bw.g_rgb + (size_t)ray * 3); g1 = __ldg(bw.g_rgb + (size_t)ray * 3 + 1); g2 = __ldg(bw.g_rgb + (size_t)ray * 3 + 2);
-                }
-                const float gd = bw.g_depth ? __ldg(bw.g_depth + ray) : 0.f;
-                const float gbg = sc.white_bkgd ? (g0 + g1 + g2) : 0.f;
-                float B = 0.f;
-                for (int j = first + S - 1; j >= first; --j) {
-                    const size_t sj = (size_t)ray * S + (j - first);
-                    const float a = sm.rgb[j * 4 + 3], Tj = s_T[j], w = a * Tj;
-                    const float c0 = sm.rgb[j * 4], c1 = sm.rgb[j * 4 + 1], c2 = sm.rgb[j * 4 + 2];
-                    float dw = g0 * c0 + g1 * c1 + g2 * c2 + gd * sm.z[j] - gbg;
-                    if (bw.g_weights) dw += __ldg(bw.g_weights + sj);
-                    float da = Tj * (dw - B);
-                    if (bw.g_alpha) da += __ldg(bw.g_alpha + sj);
-                    B = fmaf(((1.f - a) + 1e-10f), B, dw * a);
-                    s_g[j * 4 + 0] = w * g0 * c0 * (1.f - c0);
-                    s_g[j * 4 + 1] = w * g1 * c1 * (1.f - c1);
-                    s_g[j * 4 + 2] = w * g2 * c2 * (1.f - c2);
-                    s_g[j * 4 + 3] = sm.sig[j] > 0.f ? da * (1.f - a) : 0.f;
-                }
-            } else {
-                for (int j = first; j < first + S; ++j) { s_g[j * 4] = s_g[j * 4 + 1] = s_g[j * 4 + 2] = s_g[j * 4 + 3] = 0.f; }
-            }
-        }
-        if (tid >= R * S && tid < TILE_M) { s_g[tid * 4] = s_g[tid * 4 + 1] = s_g[tid * 4 + 2] = s_g[tid * 4 + 3] = 0.f; }
+        composite_scan(sc, bw, sm, s_T, s_g, grp, R, S, N, tid);
         stage_T(sm.pe, scr + bwd::S_PET, 64, tid);             // peT -> shared (used by the layer-5 and layer-0 wgrads)
         __syncthreads();
 
@@ -330,33 +396,7 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
 #pragma unroll 1
         for (int l = 5; l >= 0; --l) {
             // element-wise: acc = d h_{l+1}  ->  d g = acc * (h > 0) ; d pre = d g * mod ; d mod += d g * pre, pre = h / mod
-            {
-                const float* hT = scr + bwd::S_HT + l * 16384;
-                const float* mT = scr + bwd::S_MODT;
-#pragma unroll
-                for (int n = 0; n < 8; ++n) {
-                    const int col = frag_col(tx, n);
-#pragma unroll
-                    for (int half = 0; half < 2; ++half) {
-                        const float4 h4 = *reinterpret_cast<const float4*>(hT + col * 128 + half * 64 + ty * 4);
-                        const float4 m4 = *reinterpret_cast<const float4*>(mT + col * 128 + half * 64 + ty * 4);
-                        const float hh[4] = {h4.x, h4.y, h4.z, h4.w}, mm[4] = {m4.x, m4.y, m4.z, m4.w};
-                        float dm[4];
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int r = half * 4 + i;
-                            const bool on = hh[i] > 0.f;
-                            const float dg = on ? acc[r][n] : 0.f;
-                            acc[r][n] = dg * mm[i];
-                            dm[i] = on ? dg * __fdiv_rn(hh[i], mm[i]) : 0.f;
-                        }
-                        float4* dmod = reinterpret_cast<float4*>(scr + bwd::S_DMOD + col * 128 + half * 64 + ty * 4);
-                        float4 o = make_float4(dm[0], dm[1], dm[2], dm[3]);
-                        if (l != 5) { const float4 p = *dmod; o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w; }
-                        *dmod = o;
-                    }
-                }
-            }
+            trunk_elementwise(acc, scr, l, tid);
             frag_store_rm(acc, sm.h, H_LD, tid);
             frag_store_rm(acc, scr + bwd::S_DPRE, 128, tid);
             __syncthreads();
@@ -405,27 +445,7 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
                     *reinterpret_cast<float4*>(s_df + frag_row(ty, r) * 8 + tx * 4) = make_float4(a[r][0], a[r][1], a[r][2], a[r][3]);
             }
             __syncthreads();
-            if (tid < TILE_M && valid) {
-                // trilinear scatter (transpose of utils.index_point_feature, utils.py:357-383): same corner weights
-                float g8[8];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) g8[c] = s_df[tid * 8 + c];
-                if (bw.g_feat) {
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) g8[c] += __ldg(bw.g_feat + si * 20 + c);
-                }
-                const Trilinear t = trilinear_corners(sc, __ldg(io.ndc + si * 3), __ldg(io.ndc + si * 3 + 1), __ldg(io.ndc + si * 3 + 2));
-                const int W = sc.Wp, H = sc.Hp, D = sc.D;
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const int x = t.x0 + (c & 1), y = t.y0 + ((c >> 1) & 1), z = t.z0 + (c >> 2);
-                    if ((unsigned)x >= (unsigned)W || (unsigned)y >= (unsigned)H || (unsigned)z >= (unsigned)D) continue;   // zeros padding
-                    const float wgt = t.wx[c & 1] * t.wy[(c >> 1) & 1] * t.wz[c >> 2];
-                    float4* p = reinterpret_cast<float4*>(bw.dvol + (((size_t)z * H + y) * W + x) * 8);
-                    atomicAdd(p, make_float4(g8[0] * wgt, g8[1] * wgt, g8[2] * wgt, g8[3] * wgt));
-                    atomicAdd(p + 1, make_float4(g8[4] * wgt, g8[5] * wgt, g8[6] * wgt, g8[7] * wgt));
-                }
-            }
+            if (tid < TILE_M && valid) volume_scatter(sc, io, bw, s_df, si, tid);   // trilinear scatter
         }
         __syncthreads();
     }
@@ -488,6 +508,386 @@ __global__ void pack_dgrad_kernel(MlpPtrsB w, float* __restrict__ out) {
         for (int l = 1; l <= 4; ++l) out[bwd::D_14 + (l - 1) * 16384 + i] = w.p[2 * l][i];
     }
     for (int i = tid; i < 128 * 64; i += nt) out[bwd::D_B + i] = (i & 63) < 20 ? w.p[12][(i >> 6) * 20 + (i & 63)] : 0.f;
+}
+
+// ============================== grad_mode MVSN_MLP_TC_HALF: dgrad / wgrad on wgmma ==============================
+// render_bwd_tc_kernel is render_bwd_kernel with every trunk / feature / views / pts_bias GEMM of the backward moved
+// to wgmma with fp16 operands and fp32 accumulation.  Unchanged: the forward recompute (same fp32 tile, same
+// ScratchRecord, so rgb / depth / loss are bit-identical), the compositing scan, the element-wise stages, the bias
+// gradients (column sums of the fp32 dpre), the volume scatter and the per-CTA private accumulators.
+//
+// Operands.  Every GEMM operand is an fp16 tile in shared memory in one "core-matrix" layout: a [rows][cols] matrix
+// is stored as 8x8 blocks (128 B, one 16-byte row of 8 consecutive columns per matrix row), blocks row-major.  Read
+// as K-major (cols = K) it is a wgmma A operand; read as MN-major (rows = K, cols = N, the transposed-B form) it is
+// a B operand.  So each matrix is used in the orientation in which it is produced and no shared-memory transpose
+// exists:  wgrad  dW^T[k][n] = sum_r x^T[k][r] dpre[r][n]   A = x^T (the transposed record), B = dpre (row-major)
+//          dgrad  dx[r][k]   = sum_n dpre[r][n] W[n][k]      A = dpre,                       B = W (nn.Linear layout)
+// dpre is converted once per layer and serves as the B of the wgrad and the A of the dgrad.
+//
+// Scales.  fp16 cannot hold dpre (~1e-6 .. 1e-10 with the 1/(3 N) loss scale) nor activations (up to 1e5) as they
+// are.  Each operand tile carries an exact power-of-two scale 2^e, with e chosen so that the tile's max |v| lies in
+// [2^14, 2^15); the fp32 epilogue multiplies by 2^-(eA + eB).  Per tile and per layer, not per row: the wgrad sums
+// over rows, so a per-row scale on dpre would not factor out.  Conversions saturate at 65504, so no finite input
+// gives inf or NaN.  The weights are rounded unscaled (|w| << 65504).
+//
+// The three GEMMs of width <= 3 (rgb_linear, alpha_linear and the view-direction columns of views_linears.0) are far
+// below the wgmma N of 8; they stay FFMA on operands rounded exactly as fp16 would (round_half), so the whole
+// backward has one numerics contract: dpre, x and W rounded to an 11-bit significand, fp32 accumulation.
+//
+// Schedule: 256 threads = 2 warpgroups; warpgroup wg owns output rows [64 wg, 64 wg + 64) (or, for the 64-row
+// wgrads, output columns [64 wg, 64 wg + 64)), one m64n64k16 wgmma per 64 columns per K-step, issued back to back
+// and retired with one wait.  Tiles live in the regions the fp32 forward tile no longer needs: x16 and d16 in
+// sm.mod, the 64-row positional-encoding tile in sm.pe, the layer's fp16 weights in sm.w (cp.async from the
+// per-call fp16 image, issued at the start of the layer so the copy overlaps the element-wise stage and the
+// conversions).  Activations are converted from the same per-CTA L2 scratch the fp32 backward reads; dgrad results
+// return through sm.h (fp32, row-major) to the fragment layout of the shared element-wise code.  wgrad accumulators
+// are added straight from the wgmma registers into the private buffers (each element owned by one thread).
+namespace bwdtc {
+// fp16 dgrad weight image (halves): each B operand [K = n_out][N = k_in] in the core-matrix layout
+constexpr int W_VF = 0;                           // views_linears.0.weight[:, :128]   [64][128]
+constexpr int W_F  = W_VF + 64 * 128;             // feature_linear.weight             [128][128]
+constexpr int W_5H = W_F + 128 * 128;             // pts_linears.5.weight[:, 63:]      [128][128]
+constexpr int W_14 = W_5H + 128 * 128;            // pts_linears.1..4.weight           4 x [128][128]
+constexpr int W_B  = W_14 + 4 * 128 * 128;        // pts_bias.weight                   [128][64] (k < 20)
+constexpr int WIMG = W_B + 128 * 64;
+}  // namespace bwdtc
+
+// element (i, j) of a [rows][cols] core-matrix tile, in halves
+__host__ __device__ __forceinline__ int core_off(int i, int j, int cols) {
+    return ((i >> 3) * (cols >> 3) + (j >> 3)) * 64 + (i & 7) * 8 + (j & 7);
+}
+// saturating at +-65504 for finite values; NaN stays NaN, so a NaN operand reaches the gradients as it would in fp32
+__device__ __forceinline__ __half to_half_sat(float v) {
+    return __float2half_rn(v != v ? v : fminf(fmaxf(v, -65504.f), 65504.f));
+}
+// round to nearest even at an 11-bit significand, exponent unchanged: the value an fp16 operand carries (scaled)
+__device__ __forceinline__ float round_half(float x) {
+    const unsigned u = __float_as_uint(x);
+    return __uint_as_float((u + 0xFFFu + ((u >> 13) & 1u)) & ~0x1FFFu);
+}
+__device__ __forceinline__ float exp2i(int e) { return __int_as_float((127 + e) << 23); }   // |e| <= 126
+
+__global__ void pack_dgrad_half_kernel(MlpPtrsB w, __half* __restrict__ out) {
+    using namespace bwdtc;
+    const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
+    for (int i = tid; i < 64 * 128; i += nt) {
+        const int n = i >> 7, k = i & 127;
+        out[W_VF + core_off(n, k, 128)] = to_half_sat(w.p[14][n * 131 + k]);
+    }
+    for (int i = tid; i < 128 * 128; i += nt) {
+        const int n = i >> 7, k = i & 127, o = core_off(n, k, 128);
+        out[W_F + o] = to_half_sat(w.p[16][i]);
+        out[W_5H + o] = to_half_sat(w.p[10][n * 191 + 63 + k]);
+        for (int l = 1; l <= 4; ++l) out[W_14 + (l - 1) * 16384 + o] = to_half_sat(w.p[2 * l][i]);
+    }
+    for (int i = tid; i < 128 * 64; i += nt) {
+        const int n = i >> 6, k = i & 63;
+        out[W_B + core_off(n, k, 64)] = to_half_sat(k < 20 ? w.p[12][n * 20 + k] : 0.f);
+    }
+}
+
+// Block-wide max |v| -> the exponent e of the tile's scale 2^e (max * 2^e in [2^14, 2^15); e = 0 for an all-zero
+// tile; clamped to +-62 so that 2^-(eA + eB) is a normal float).  Three rotating slots: use i reads slot i % 3
+// after the barrier and clears slot (i + 2) % 3, whose last reader passed the barrier of use i and whose next writer
+// comes after the barrier of use i + 1.
+__device__ __forceinline__ int block_scale_exp(float m, unsigned* s_amax, int& i, int tid) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((tid & 31) == 0) atomicMax(s_amax + i % 3, __float_as_uint(m));
+    __syncthreads();
+    const unsigned b = s_amax[i % 3];
+    if (tid == 0) s_amax[(i + 2) % 3] = 0u;
+    ++i;
+    if (b == 0u) return 0;
+    const int e = 14 - ((int)(b >> 23) - 127);
+    return e < -62 ? -62 : (e > 62 ? 62 : e);
+}
+
+// fp32 [rows][cols] (row stride ld floats, shared or global) -> scaled fp16 core-matrix tile; returns the exponent.
+// Ends with the tile visible to wgmma (proxy fence + barrier).
+__device__ __forceinline__ int stage_half(const float* src, int ld, int rows, int cols, __half* dst, unsigned* s_amax,
+                                          int& amax_i, int tid) {
+    const int upr = cols >> 3, units = rows * upr;
+    float m = 0.f;
+    for (int u = tid; u < units; u += 256) {
+        const float* p = src + (u / upr) * ld + (u % upr) * 8;
+        const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+        m = fmaxf(m, fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))),
+                           fmaxf(fmaxf(fabsf(b.x), fabsf(b.y)), fmaxf(fabsf(b.z), fabsf(b.w)))));
+    }
+    const int e = block_scale_exp(m, s_amax, amax_i, tid);
+    const float s = exp2i(e);
+    for (int u = tid; u < units; u += 256) {
+        const int r = u / upr, c8 = u % upr;
+        const float* p = src + r * ld + c8 * 8;
+        const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+        __half2 h[4] = {__halves2half2(to_half_sat(a.x * s), to_half_sat(a.y * s)), __halves2half2(to_half_sat(a.z * s), to_half_sat(a.w * s)),
+                        __halves2half2(to_half_sat(b.x * s), to_half_sat(b.y * s)), __halves2half2(to_half_sat(b.z * s), to_half_sat(b.w * s))};
+        *reinterpret_cast<uint4*>(dst + core_off(r, c8 * 8, cols)) = *reinterpret_cast<const uint4*>(h);
+    }
+    hop::fence_proxy_async();
+    __syncthreads();
+    return e;
+}
+
+// fp16 weight operand (a contiguous slice of the image) -> sm.w by cp.async; completed by load_w_wait
+__device__ __forceinline__ void load_w_issue(const __half* src, int halves, __half* dst, int tid) {
+    for (int i = tid; i < halves / 8; i += 256) cp_async16(dst + i * 8, src + i * 8);
+    cp_async_commit();
+}
+__device__ __forceinline__ void load_w_wait() {
+    cp_async_wait<0>();
+    hop::fence_proxy_async();
+    __syncthreads();
+}
+
+// d[h] = this warpgroup's 64 rows x columns [64 h, 64 h + 64) of A[.][K] * B[K][.]:  a = the warpgroup's first A row
+// (core-matrix tile with K columns), b = its first B column (core-matrix tile with ncols columns).
+template <int NH, int K>
+__device__ __forceinline__ void tc_gemm(float (&d)[NH][32], const __half* a, const __half* b, int ncols) {
+    const uint32_t sa = hop::smem_u32(a), sb = hop::smem_u32(b);
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) d[h][i] = 0.f;
+    hop::wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < K / 16; ++ks) {
+        const uint64_t da = hop::desc_nosw(sa + ks * 256, 128, K * 16);
+#pragma unroll
+        for (int h = 0; h < NH; ++h)
+            hop::WgmmaTB<64>::ss(d[h], da, hop::desc_nosw(sb + ks * 32 * ncols + h * 1024, ncols * 16, 128), 1);
+    }
+    hop::wgmma_commit();
+    hop::wgmma_wait<0>();
+#pragma unroll
+    for (int h = 0; h < NH; ++h) hop::reg_fence(d[h]);
+}
+
+// accumulator -> row-major fp32 [.][ld] (ACC: += into a private gradient buffer; else: store), times `scale`.
+// Element d[h][4 j + 2 hh + e] is row row0 + 16 w + g + 8 hh, column col0 + 64 h + 8 j + 2 q + e.
+template <bool ACC, int NH>
+__device__ __forceinline__ void tc_write(const float (&d)[NH][32], float scale, float* dst, int ld, int row0, int col0, int tid) {
+    const int t = tid & 127, w = t >> 5, g = (t >> 2) & 7, q = t & 3;
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                float2* p = reinterpret_cast<float2*>(dst + (row0 + 16 * w + g + 8 * hh) * ld + col0 + 64 * h + 8 * j + 2 * q);
+                float2 v = make_float2(d[h][4 * j + 2 * hh] * scale, d[h][4 * j + 2 * hh + 1] * scale);
+                if (ACC) { const float2 o = *p; v.x += o.x; v.y += o.y; }
+                *p = v;
+            }
+}
+
+// row-major fp32 [128][H_LD] (shared) -> the thread's fragment; barriers on both sides, so the caller may overwrite
+// the source right after
+__device__ __forceinline__ void frag_load_rm(float (&acc)[8][8], const float* src, int tid) {
+    const int ty = tid >> 4, tx = tid & 15;
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+        const float* p = src + frag_row(ty, r) * H_LD + tx * 4;
+        const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 64);
+        acc[r][0] = a.x; acc[r][1] = a.y; acc[r][2] = a.z; acc[r][3] = a.w;
+        acc[r][4] = b.x; acc[r][5] = b.y; acc[r][6] = b.z; acc[r][7] = b.w;
+    }
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(256, 1)
+render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts,
+                     const __half* __restrict__ wh) {
+    using namespace bwdtc;
+    extern __shared__ __align__(16) float smem[];
+    const TileSmem sm(smem);
+    float* s_T    = sm.tail;
+    float* s_g    = s_T + TILE_M;
+    float* s_df   = s_g + TILE_M * 4;
+    __half* pe16  = reinterpret_cast<__half*>(sm.pe);         // [64][128]  peT: A of the layer-5 / layer-0 pe wgrads
+    __half* x16   = reinterpret_cast<__half*>(sm.mod);        // [<=128][128] x^T: A of the wgrads
+    __half* d16   = x16 + 128 * 128;                           // [128][<=128] dpre: B of the wgrads, A of the dgrads
+    __half* w16   = reinterpret_cast<__half*>(sm.w);          // [<=128][128] W: B of the dgrads
+    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15, wg = tid >> 7;
+    __shared__ Cams cams;
+    __shared__ unsigned s_amax[3];
+    load_cams(sc, &cams, tid);
+    if (tid < 3) s_amax[tid] = 0u;
+    int amax_i = 0;
+
+    float* scr = bw.scratch + (size_t)blockIdx.x * bwd::SCRATCH;
+    float* G = bw.grads + (size_t)blockIdx.x * bwd::GRADS;
+    for (int i = tid; i < bwd::GRADS; i += 256) G[i] = 0.f;
+    for (int i = tid; i < 32 * 128; i += 256) scr[bwd::S_FEATT + 32 * 128 + i] = 0.f;
+    __syncthreads();
+
+    const int N = io.N, S = io.S;
+    const int R = TILE_M / S;
+    const int ngroups = (N + R - 1) / R;
+
+    for (int grp = blockIdx.x; grp < ngroups; grp += gridDim.x) {
+        // =============================== forward recompute (the fp32 tile) ===========================
+        bool valid = false;
+        size_t si = 0;
+        if (tid < TILE_M) {
+            const int r_in = tid / S, s_idx = tid - r_in * S, ray = grp * R + r_in;
+            valid = r_in < R && ray < N;
+            si = (size_t)ray * S + s_idx;
+            tile_front_end<false>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr});
+        }
+        __syncthreads();
+        tile_mlp(sm, wts, tid, ScratchRecord{scr});
+        __syncthreads();
+        composite_scan(sc, bw, sm, s_T, s_g, grp, R, S, N, tid);
+        load_w_issue(wh + W_VF, 64 * 128, w16, tid);
+        __syncthreads();
+        const int e_pe = stage_half(scr + bwd::S_PET, 128, 64, 128, pe16, s_amax, amax_i, tid);
+
+        // =============================== heads (N <= 3: FFMA on fp16-rounded operands) ================
+        if (tid < 64) {
+            float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+            for (int r = 0; r < TILE_M; ++r) {
+                const float h = round_half(sm.mod[r * HV_LD + tid]);
+                a0 = fmaf(round_half(s_g[r * 4]), h, a0); a1 = fmaf(round_half(s_g[r * 4 + 1]), h, a1);
+                a2 = fmaf(round_half(s_g[r * 4 + 2]), h, a2);
+            }
+            G[bwd::G_WR + tid] += a0; G[bwd::G_WR + 64 + tid] += a1; G[bwd::G_WR + 128 + tid] += a2;
+        } else if (tid < 68) {
+            const int c = tid - 64;
+            float a = 0.f;
+            for (int r = 0; r < TILE_M; ++r) a += s_g[r * 4 + c];
+            G[bwd::G_BR + c] += a;
+        }
+        {
+            // d hv_pre[r][j] = (hv > 0) * sum_c d rgb_pre[r][c] Wr[c][j]  -> sm.h (fp32, row-major)
+            const float4 w0 = __ldg(reinterpret_cast<const float4*>(wts + w32::WR + tx * 4));
+            const float4 w1 = __ldg(reinterpret_cast<const float4*>(wts + w32::WR + 64 + tx * 4));
+            const float4 w2 = __ldg(reinterpret_cast<const float4*>(wts + w32::WR + 128 + tx * 4));
+            const float wr[3][4] = {{round_half(w0.x), round_half(w0.y), round_half(w0.z), round_half(w0.w)},
+                                    {round_half(w1.x), round_half(w1.y), round_half(w1.z), round_half(w1.w)},
+                                    {round_half(w2.x), round_half(w2.y), round_half(w2.z), round_half(w2.w)}};
+#pragma unroll
+            for (int r = 0; r < 8; ++r) {
+                const int row = frag_row(ty, r);
+                const float d0 = round_half(s_g[row * 4]), d1 = round_half(s_g[row * 4 + 1]), d2 = round_half(s_g[row * 4 + 2]);
+                const float4 hv = *reinterpret_cast<const float4*>(sm.mod + row * HV_LD + tx * 4);
+                const float hvv[4] = {hv.x, hv.y, hv.z, hv.w};
+                float o[4];
+#pragma unroll
+                for (int c = 0; c < 4; ++c) o[c] = hvv[c] > 0.f ? fmaf(d2, wr[2][c], fmaf(d1, wr[1][c], d0 * wr[0][c])) : 0.f;
+                *reinterpret_cast<float4*>(sm.h + row * H_LD + tx * 4) = make_float4(o[0], o[1], o[2], o[3]);
+            }
+        }
+        __syncthreads();                                        // hv (sm.mod) no longer needed; d hv_pre complete
+        if (tid < 64) {                                         // d bv, d Wv[:, 128:131]^T
+            float sb = 0.f, s0 = 0.f, s1 = 0.f, s2 = 0.f;
+            for (int r = 0; r < TILE_M; ++r) {
+                const float d = sm.h[r * H_LD + tid], dr = round_half(d);
+                sb += d;
+                s0 = fmaf(round_half(sm.dir[r * 4]), dr, s0); s1 = fmaf(round_half(sm.dir[r * 4 + 1]), dr, s1);
+                s2 = fmaf(round_half(sm.dir[r * 4 + 2]), dr, s2);
+            }
+            G[bwd::G_BV + tid] += sb;
+            G[bwd::G_WVDT + tid] += s0; G[bwd::G_WVDT + 64 + tid] += s1; G[bwd::G_WVDT + 128 + tid] += s2;
+        }
+        const int e_dv = stage_half(sm.h, H_LD, 128, 64, d16, s_amax, amax_i, tid);
+        const int e_f = stage_half(scr + bwd::S_FT, 128, 128, 128, x16, s_amax, amax_i, tid);
+        float d[2][32];
+        {
+            float d1[1][32];                                    // d Wv_f^T[k][j] = sum_r fT[k][r] d hv_pre[r][j]
+            tc_gemm<1, 128>(d1, x16 + wg * 64 * 128, d16, 64);
+            tc_write<true>(d1, exp2i(-(e_f + e_dv)), G + bwd::G_WVFT, 64, 64 * wg, 0, tid);
+        }
+        load_w_wait();                                          // d f[r][k] = sum_j d hv_pre[r][j] Wv[j][k]
+        tc_gemm<2, 64>(d, d16 + wg * 64 * 64, w16, 128);
+        tc_write<false>(d, exp2i(-e_dv), sm.h, H_LD, 64 * wg, 0, tid);
+        __syncthreads();
+        load_w_issue(wh + W_F, 128 * 128, w16, tid);
+        colsum_accumulate(sm.h, H_LD, 128, G + bwd::G_BF, tid); // d bf
+        const int e_df = stage_half(sm.h, H_LD, 128, 128, d16, s_amax, amax_i, tid);
+        const int e_h6 = stage_half(scr + bwd::S_HT + 5 * 16384, 128, 128, 128, x16, s_amax, amax_i, tid);
+        tc_gemm<2, 128>(d, x16 + wg * 64 * 128, d16, 128);      // d Wf^T[k][n] = sum_r h6T[k][r] d f[r][n]
+        tc_write<true>(d, exp2i(-(e_h6 + e_df)), G + bwd::G_WFT, 128, 64 * wg, 0, tid);
+        if (tid < TILE_M) {                                     // d wa[k] = sum_r d sigma_pre[r] h6T[k][r]
+            const float* h6 = scr + bwd::S_HT + 5 * 16384 + tid * 128;
+            float s = 0.f;
+            for (int r = 0; r < TILE_M; ++r) s = fmaf(round_half(s_g[r * 4 + 3]), round_half(h6[r]), s);
+            G[bwd::G_WA + tid] += s;
+        }
+        load_w_wait();                                          // d h6 = d f Wf + d sigma_pre (x) wa
+        tc_gemm<2, 128>(d, d16 + wg * 64 * 128, w16, 128);
+        tc_write<false>(d, exp2i(-e_df), sm.h, H_LD, 64 * wg, 0, tid);
+        float acc[8][8];
+        frag_load_rm(acc, sm.h, tid);
+        {
+            const float4 al = __ldg(reinterpret_cast<const float4*>(wts + w32::WA + tx * 4));
+            const float4 ah = __ldg(reinterpret_cast<const float4*>(wts + w32::WA + 64 + tx * 4));
+            const float wa[8] = {round_half(al.x), round_half(al.y), round_half(al.z), round_half(al.w),
+                                 round_half(ah.x), round_half(ah.y), round_half(ah.z), round_half(ah.w)};
+#pragma unroll
+            for (int r = 0; r < 8; ++r) {
+                const float ds = round_half(s_g[frag_row(ty, r) * 4 + 3]);
+#pragma unroll
+                for (int n = 0; n < 8; ++n) acc[r][n] = fmaf(ds, wa[n], acc[r][n]);
+            }
+        }
+
+        // =============================== trunk, layers 5..0 ==========================================
+#pragma unroll 1
+        for (int l = 5; l >= 0; --l) {
+            trunk_elementwise(acc, scr, l, tid);
+            frag_store_rm(acc, sm.h, H_LD, tid);
+            if (l >= 1) load_w_issue(wh + (l == 5 ? W_5H : W_14 + (l - 1) * 16384), 128 * 128, w16, tid);
+            __syncthreads();
+            colsum_accumulate(sm.h, H_LD, 128, G + bwd::G_B + l * 128, tid);                 // d b_l
+            const int e_d = stage_half(sm.h, H_LD, 128, 128, d16, s_amax, amax_i, tid);
+            if (l >= 1) {                                       // d W_l^T[k][n] = sum_r h_l^T[k][r] d pre[r][n]
+                const int e_x = stage_half(scr + bwd::S_HT + (l - 1) * 16384, 128, 128, 128, x16, s_amax, amax_i, tid);
+                tc_gemm<2, 128>(d, x16 + wg * 64 * 128, d16, 128);
+                tc_write<true>(d, exp2i(-(e_x + e_d)), G + (l == 5 ? bwd::G_W5HT : bwd::G_W14T + (l - 1) * 16384), 128, 64 * wg, 0, tid);
+            }
+            if (l == 5 || l == 0) {                             // positional-encoding part: 64-row A, column half per warpgroup
+                float d1[1][32];
+                tc_gemm<1, 128>(d1, pe16, d16 + wg * 512, 128);
+                tc_write<true>(d1, exp2i(-(e_pe + e_d)), G + (l == 5 ? bwd::G_W5PET : bwd::G_W0T), 128, 0, 64 * wg, tid);
+            }
+            if (l >= 1) {                                       // d h_l = d pre W_l (h part)
+                load_w_wait();
+                tc_gemm<2, 128>(d, d16 + wg * 64 * 128, w16, 128);
+                tc_write<false>(d, exp2i(-e_d), sm.h, H_LD, 64 * wg, 0, tid);
+                frag_load_rm(acc, sm.h, tid);
+            }
+        }
+        // =============================== modulation branch: pts_bias ==================================
+        frag_load_T(acc, scr + bwd::S_DMOD, tid);
+        frag_store_rm(acc, sm.h, H_LD, tid);
+        if (bw.dvol) load_w_issue(wh + W_B, 128 * 64, w16, tid);
+        __syncthreads();
+        colsum_accumulate(sm.h, H_LD, 128, G + bwd::G_BB, tid);
+        const int e_m = stage_half(sm.h, H_LD, 128, 128, d16, s_amax, amax_i, tid);
+        const int e_ft = stage_half(scr + bwd::S_FEATT, 128, 64, 128, x16, s_amax, amax_i, tid);
+        {
+            float d1[1][32];                                    // d Wb^T[k][n] = sum_r featT[k][r] d mod[r][n]
+            tc_gemm<1, 128>(d1, x16, d16 + wg * 512, 128);
+            tc_write<true>(d1, exp2i(-(e_ft + e_m)), G + bwd::G_WBT, 128, 0, 64 * wg, tid);
+        }
+        if (bw.dvol) {
+            load_w_wait();                                      // d feat[r][k] = sum_n d mod[r][n] Wb[n][k], k < 8
+            float d1[1][32];
+            tc_gemm<1, 128>(d1, d16 + wg * 64 * 128, w16, 64);
+            const int t = tid & 127, w = t >> 5, g = (t >> 2) & 7, q = t & 3;
+            const float sc_m = exp2i(-e_m);
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+                *reinterpret_cast<float2*>(s_df + (64 * wg + 16 * w + g + 8 * hh) * 8 + 2 * q) =
+                    make_float2(d1[0][2 * hh] * sc_m, d1[0][2 * hh + 1] * sc_m);
+            __syncthreads();
+            if (tid < TILE_M && valid) volume_scatter(sc, io, bw, s_df, si, tid);
+        }
+        __syncthreads();
+    }
 }
 
 // ---- fused Adam (torch.optim.Adam: no weight decay, no amsgrad) ---------------------------------------------
@@ -559,21 +959,29 @@ size_t render_backward_workspace_bytes(int N, int S) {
     return (ctas * (bwd::SCRATCH + bwd::GRADS) + bwd::DGRAD) * sizeof(float);
 }
 
+size_t render_backward_tc_workspace_bytes(int N, int S) {
+    if (S <= 0 || S > TILE_M || N <= 0) return 0;
+    const size_t ctas = (size_t)sm_count();
+    return ctas * (bwd::SCRATCH + bwd::GRADS) * sizeof(float) + bwdtc::WIMG * sizeof(__half);
+}
+
 int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const float* const* mlp_w,
                            const float* g_rgb, const float* target, float inv_count, const float* g_depth,
                            const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
                            float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream) {
-    MVSN_REQUIRE(io.S <= TILE_M, MVSN_EUNSUPPORTED, "render backward: N_samples=%d > 128 is not implemented", io.S);
-    const size_t need = render_backward_workspace_bytes(io.N, io.S);
-    MVSN_REQUIRE(workspace && workspace_bytes >= need, MVSN_EWORKSPACE, "render backward: workspace %zu < %zu bytes", workspace_bytes, need);
-    MVSN_REQUIRE(aligned16(workspace), MVSN_EALIGN, "render backward: workspace must be 16-byte aligned");
-    static bool attr_set[64] = {false};
+                           size_t workspace_bytes, cudaStream_t stream, bool tc) {
+    const char* what = tc ? "render backward (grad_mode TC_HALF)" : "render backward";
+    MVSN_REQUIRE(io.S <= TILE_M, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, io.S);
+    const size_t need = tc ? render_backward_tc_workspace_bytes(io.N, io.S) : render_backward_workspace_bytes(io.N, io.S);
+    MVSN_REQUIRE(workspace && workspace_bytes >= need, MVSN_EWORKSPACE, "%s: workspace %zu < %zu bytes", what, workspace_bytes, need);
+    MVSN_REQUIRE(aligned16(workspace), MVSN_EALIGN, "%s: workspace must be 16-byte aligned", what);
+    static bool attr_set[2][64] = {};
     int dev = 0;
     MVSN_CUDA_CHECK(cudaGetDevice(&dev));
-    if (dev >= 64 || !attr_set[dev]) {
-        MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
-        if (dev < 64) attr_set[dev] = true;
+    if (dev >= 64 || !attr_set[tc][dev]) {
+        if (tc) MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+        else    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+        if (dev < 64) attr_set[tc][dev] = true;
     }
     const int grid = bwd_grid(io.N, io.S);
     float* ws = static_cast<float*>(workspace);
@@ -582,13 +990,20 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
     bw.g_rgb = g_rgb; bw.target = target; bw.inv_count = inv_count; bw.g_depth = g_depth; bw.g_weights = g_weights;
     bw.g_alpha = g_alpha; bw.g_feat = g_feat; bw.dvol = dvol; bw.rgb_out = rgb_out; bw.depth_out = depth_out; bw.loss = loss;
     bw.scratch = ws; bw.grads = ws + ctas * bwd::SCRATCH;
-    float* wd = ws + ctas * (bwd::SCRATCH + bwd::GRADS);
-    bw.wd = wd;
+    float* wimg = ws + ctas * (bwd::SCRATCH + bwd::GRADS);   // the dgrad weight image: fp32, or fp16 for the tc kernel
     MlpPtrsB wp;
     for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) wp.p[i] = mlp_w[i];
-    pack_dgrad_kernel<<<64, 256, 0, stream>>>(wp, wd);
-    MVSN_CUDA_CHECK(cudaGetLastError());
-    render_bwd_kernel<<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32);
+    if (tc) {
+        __half* wh = reinterpret_cast<__half*>(wimg);
+        pack_dgrad_half_kernel<<<64, 256, 0, stream>>>(wp, wh);
+        MVSN_CUDA_CHECK(cudaGetLastError());
+        render_bwd_tc_kernel<<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, wh);
+    } else {
+        bw.wd = wimg;
+        pack_dgrad_kernel<<<64, 256, 0, stream>>>(wp, wimg);
+        MVSN_CUDA_CHECK(cudaGetLastError());
+        render_bwd_kernel<<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32);
+    }
     MVSN_CUDA_CHECK(cudaGetLastError());
     GradOut go;
     for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) go.p[i] = grad_mlp[i];
