@@ -183,6 +183,23 @@ int mvsn_render_backward_tc(const mvsn_render_scene* scene, const float* const* 
                             const float* rays_pts, const float* rays_ndc, const float* z_vals, const float* rays_dir,
                             int N, int S, const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc,
                             void* workspace, size_t workspace_bytes, void* stream);
+/* mvsn_render_backward_deterministic: mvsn_render_backward (grad_mode MVSN_MLP_FP32) or mvsn_render_backward_tc
+ * (MVSN_MLP_TC_HALF) with every output bit-reproducible from call to call on the same GPU model and inputs.  The
+ * backward kernel records each sample's 8 volume-feature gradients and each ray's loss term instead of adding them
+ * with float atomics; the volume gradient is then summed as 64-bit fixed-point integers at a power-of-two scale chosen
+ * from the largest |gradient| (contributions below ~max|g| * N * S * 2^-62 round to zero) and ACCUMULATED into
+ * grad_volume_dhwc, and loss_out is ACCUMULATED with the per-ray terms summed in a fixed order.  rgb_out / depth_out
+ * and the MLP gradients are the same as the non-deterministic entry's.  A non-finite gradient makes the volume
+ * entries it touches NaN / inf as the atomics would.  Any other grad_mode: MVSN_EUNSUPPORTED, before any CUDA call.
+ * Workspace: mvsn_render_backward_deterministic_workspace_bytes(N, S, D, Hp, Wp, grad_mode), 16-byte aligned, with the
+ * scene's volume dims (it holds a [D,Hp,Wp,8] int64 accumulator, zeroed by every call); D = Hp = Wp = 0 sizes it for a
+ * frozen volume (grad_volume_dhwc = NULL).  0 for an unknown grad_mode or shape. */
+size_t mvsn_render_backward_deterministic_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode);
+int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const float* const* mlp_w,
+                                       const float* rays_pts, const float* rays_ndc, const float* z_vals,
+                                       const float* rays_dir, int N, int S, int grad_mode, const mvsn_render_grads* g,
+                                       float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
+                                       size_t workspace_bytes, void* stream);
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
                    const int* numel_host, int count, float lr, float beta1, float beta2, float eps, int step,
                    void* stream);

@@ -554,8 +554,8 @@ class _RenderSamplesFn(torch.autograd.Function):
     backward: gradients w.r.t. the 22 MLP tensors and the encoding volume.  With N_samples <= 128 (and
     BACKWARD_IMPL == "kernel") they come from the backward kernel (csrc/render_bwd.cu: forward recompute on the
     fp32 render kernel's own forward tile, MLP dgrad/wgrad in the arithmetic `grad_mode` selects, trilinear scatter
-    into the volume gradient).  Otherwise
-    the chunk is re-evaluated with PyTorch ops under autograd (_render_samples_torch); activation memory then
+    into the volume gradient; bit-reproducible under torch.use_deterministic_algorithms(True), see render_backward).
+    Otherwise the chunk is re-evaluated with PyTorch ops under autograd (_render_samples_torch); activation memory then
     exists only during backward."""
 
     @staticmethod
@@ -612,9 +612,14 @@ def _check_grad_mode(grad_mode):
                            "(wgmma, fp16 operands with per-tile power-of-two scales, fp32 accumulation)")
 
 
-def _backward_workspace(dev, N, S, grad_mode=_lib.MLP_FP32):
+def _backward_workspace(dev, N, S, grad_mode=_lib.MLP_FP32, det_volume=None):
+    """The shared backward workspace, grown to this call's need.  det_volume = (D, Hp, Wp) of the volume gradient, or
+    (0, 0, 0) for a frozen volume, sizes it for mvsn_render_backward_deterministic instead."""
     lib = _lib.load()
-    if grad_mode == _lib.MLP_TC_HALF:
+    if det_volume is not None:
+        need = lib.mvsn_render_backward_deterministic_workspace_bytes(int(N), int(S), *[int(v) for v in det_volume],
+                                                                     int(grad_mode))
+    elif grad_mode == _lib.MLP_TC_HALF:
         need = lib.mvsn_render_backward_tc_workspace_bytes(int(N), int(S))
     else:
         need = lib.mvsn_render_backward_workspace_bytes(int(N), int(S))
@@ -636,7 +641,11 @@ def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_featu
     'input_feat': d loss / d output of `rendering`) or `target_rgb` [N,3] (img2mse formed in the kernel, normalised by
     3 * n_total).  Returns (grad_mlp[22] in ordered_params() order, grad_volume [D,Hp,Wp,8] channels-last or None,
     rgb [N,3] or None, depth [N] or None).  `grad_volume` (accumulated into) and `grad_mlp` (overwritten) may be passed
-    to reuse buffers."""
+    to reuse buffers.
+
+    With torch.use_deterministic_algorithms(True) in effect at call time the launch is
+    mvsn_render_backward_deterministic instead (same grad_mode): the volume gradient and the fused loss are summed in
+    a fixed order, so every output is bit-reproducible; otherwise they are summed with float atomics."""
     _check_grad_mode(grad_mode)
     lib = _lib.load()
     N, S = rays_pts.shape[:2]
@@ -682,13 +691,22 @@ def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_featu
         g.rgb_out, g.depth_out = rgb.data_ptr(), depth.data_ptr()
     if loss_out is not None:
         g.loss_out = loss_out.data_ptr()
+    vol_arg = _lib.ptr(grad_volume) if want_volume_grad else None
+    if torch.are_deterministic_algorithms_enabled():
+        ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode, (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0))
+        with torch.cuda.device(dev):
+            _lib.check(lib.mvsn_render_backward_deterministic(
+                C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z), _lib.ptr(dirs), N, S,
+                int(grad_mode), C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(ws), ws_bytes,
+                _lib.stream_ptr()), "mvsn_render_backward_deterministic")
+        del keep, held
+        return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
     ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode)
     entry, name = ((lib.mvsn_render_backward_tc, "mvsn_render_backward_tc") if grad_mode == _lib.MLP_TC_HALF
                    else (lib.mvsn_render_backward, "mvsn_render_backward"))
     with torch.cuda.device(dev):
         _lib.check(entry(C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z),
-                         _lib.ptr(dirs), N, S, C.byref(g), _lib.ptr_array(grad_mlp),
-                         _lib.ptr(grad_volume) if want_volume_grad else None, _lib.ptr(ws), ws_bytes,
+                         _lib.ptr(dirs), N, S, C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(ws), ws_bytes,
                          _lib.stream_ptr()), name)
     del keep, held
     return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
@@ -703,7 +721,9 @@ class FineTuner:
 
     The parameters stay the caller's nn.Parameters (updated in place, version counters bumped), so checkpoints, the
     render entry points and scene_io see them as after a torch.optim.Adam step with the same hyper-parameters.
-    grad_mode=MLP_TC_HALF runs the backward's dgrad / wgrad GEMMs on tensor cores (see render_backward)."""
+    grad_mode=MLP_TC_HALF runs the backward's dgrad / wgrad GEMMs on tensor cores (see render_backward).  Under
+    torch.use_deterministic_algorithms(True) every step is bit-reproducible: two runs from the same start on the same
+    batches end with identical parameters, volume and losses (see render_backward)."""
 
     def __init__(self, network_fn, volume, imgs, pose_ref, lr=5e-4, betas=(0.9, 0.999), eps=1e-8, white_bkgd=False,
                  grad_mode=_lib.MLP_FP32):

@@ -309,11 +309,15 @@ int mvsn_make_rays(const float* directions, const float* c2w, float near, float 
 // ---- fine-tuning step ------------------------------------------------------------------------------------
 size_t mvsn_render_backward_workspace_bytes(int N, int S) { return render_backward_workspace_bytes(N, S); }
 size_t mvsn_render_backward_tc_workspace_bytes(int N, int S) { return render_backward_tc_workspace_bytes(N, S); }
+size_t mvsn_render_backward_deterministic_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode) {
+    if (grad_mode != MVSN_MLP_FP32 && grad_mode != MVSN_MLP_TC_HALF) return 0;
+    return render_backward_det_workspace_bytes(N, S, D, Hp, Wp, grad_mode == MVSN_MLP_TC_HALF);
+}
 
 static int render_backward_entry(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
                                  const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
                                  const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc,
-                                 void* workspace, size_t workspace_bytes, void* stream, bool tc) {
+                                 void* workspace, size_t workspace_bytes, void* stream, bool tc, bool det = false) {
     SceneDev sc;
     int rc = make_scene(scene, sc);
     if (rc) return rc;
@@ -333,7 +337,7 @@ static int render_backward_entry(const mvsn_render_scene* scene, const float* co
     return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
                                   g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
                                   grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
-                                  (cudaStream_t)stream, tc);
+                                  (cudaStream_t)stream, tc, det);
 }
 
 int mvsn_render_backward(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
@@ -352,6 +356,17 @@ int mvsn_render_backward_tc(const mvsn_render_scene* scene, const float* const* 
     MVSN_RANGE("mvsn_render_backward_tc");
     return render_backward_entry(scene, mlp_w, rays_pts, rays_ndc, z_vals, rays_dir, N, S, g, grad_mlp, grad_volume_dhwc,
                                  workspace, workspace_bytes, stream, true);
+}
+
+int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                                       const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                                       int grad_mode, const mvsn_render_grads* g, float* const* grad_mlp,
+                                       float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward_deterministic");
+    MVSN_REQUIRE(grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF, MVSN_EUNSUPPORTED,
+                 "mvsn_render_backward_deterministic: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)", grad_mode);
+    return render_backward_entry(scene, mlp_w, rays_pts, rays_ndc, z_vals, rays_dir, N, S, g, grad_mlp, grad_volume_dhwc,
+                                 workspace, workspace_bytes, stream, grad_mode == MVSN_MLP_TC_HALF, true);
 }
 
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,

@@ -27,6 +27,12 @@
 //
 // grad_mode MVSN_MLP_TC_HALF (mvsn_render_backward_tc) runs render_bwd_tc_kernel instead: the same tile with its
 // dgrad / wgrad GEMMs on wgmma with fp16 operands; its schedule and numerics are described above the kernel.
+//
+// mvsn_render_backward_deterministic runs either kernel with DET = true: the volume scatter and the fused loss are
+// recorded instead of summed with float atomics, then summed in a fixed-point scatter and a fixed-order reduction
+// (described above det_scatter_kernel), so every output is bit-reproducible.
+#include <cfloat>
+
 #include "tile_fp32.cuh"
 #include "hopper.cuh"
 
@@ -83,6 +89,13 @@ struct BwdIO {
     float* rgb_out;          // [N,3] optional: the forward result of the recompute
     float* depth_out;        // [N]   optional
     float* loss;             // [1]   optional: += sum (rgb - target)^2 * inv_count
+};
+
+// What the DET = true kernels record instead of adding atomically (mvsn_render_backward_deterministic)
+struct DetIO {
+    float* rec;              // [N*S][8] each sample's 8 volume-feature gradients (null: the volume is frozen)
+    float* loss_terms;       // [N] each ray's loss term (with bw.loss)
+    unsigned* amax;          // [2] max |g| over the finite recorded values (float bits), and a non-finite flag
 };
 
 namespace {
@@ -163,8 +176,10 @@ static_assert(TILE_M * PE_LD >= 64 * H_LD, "peT staging [64][H_LD] must fit in t
 // depth_out / the fused loss, s_T (transmittance in front of each sample) and s_g (d rgb_pre, d sigma_pre per row).
 // f_j = 1 - alpha_j + 1e-10, T_{j+1} = T_j f_j, w_j = alpha_j T_j.
 // d alpha_j = T_j (d w_j - B_j),  B_{j-1} = d w_j alpha_j + f_j B_j  (no division by f_j).
+// DET: the ray's loss term goes to det.loss_terms[ray] instead of being added to bw.loss.
+template <bool DET>
 __device__ __forceinline__ void composite_scan(const SceneDev& sc, const BwdIO& bw, const TileSmem& sm, float* s_T, float* s_g,
-                                               int grp, int R, int S, int N, int tid) {
+                                               int grp, int R, int S, int N, int tid, const DetIO& det) {
     if (tid < R) {
         const int ray = grp * R + tid, first = tid * S;
         if (ray < N) {
@@ -184,7 +199,10 @@ __device__ __forceinline__ void composite_scan(const SceneDev& sc, const BwdIO& 
                 const float e0 = cr - __ldg(bw.target + (size_t)ray * 3), e1 = cg - __ldg(bw.target + (size_t)ray * 3 + 1),
                             e2 = cb - __ldg(bw.target + (size_t)ray * 3 + 2);
                 g0 = 2.f * e0 * bw.inv_count; g1 = 2.f * e1 * bw.inv_count; g2 = 2.f * e2 * bw.inv_count;
-                if (bw.loss) atomicAdd(bw.loss, (e0 * e0 + e1 * e1 + e2 * e2) * bw.inv_count);
+                if (bw.loss) {
+                    if constexpr (DET) det.loss_terms[ray] = (e0 * e0 + e1 * e1 + e2 * e2) * bw.inv_count;
+                    else               atomicAdd(bw.loss, (e0 * e0 + e1 * e1 + e2 * e2) * bw.inv_count);
+                }
             } else {
                 g0 = __ldg(bw.g_rgb + (size_t)ray * 3); g1 = __ldg(bw.g_rgb + (size_t)ray * 3 + 1); g2 = __ldg(bw.g_rgb + (size_t)ray * 3 + 2);
             }
@@ -245,14 +263,37 @@ __device__ __forceinline__ void trunk_elementwise(float (&acc)[8][8], float* scr
 
 // Trilinear scatter of row `tid`'s 8 volume-feature gradients (s_df, plus d input_feat) into the channels-last volume
 // gradient: the transpose of utils.index_point_feature (utils.py:357-383), with the same corner weights.
+// DET: the 8 gradients are recorded to det.rec[si] and folded into det.amax (max |g| over the finite values, as float
+// bits with an integer atomicMax, so the result does not depend on the order; any non-finite value sets amax[1]);
+// det_scatter_kernel scatters them afterwards.  The caller is divergent (valid rows only), hence __activemask.
+template <bool DET>
 __device__ __forceinline__ void volume_scatter(const SceneDev& sc, const RenderIO& io, const BwdIO& bw, const float* s_df,
-                                               size_t si, int tid) {
+                                               size_t si, int tid, const DetIO& det) {
     float g8[8];
 #pragma unroll
     for (int c = 0; c < 8; ++c) g8[c] = s_df[tid * 8 + c];
     if (bw.g_feat) {
 #pragma unroll
         for (int c = 0; c < 8; ++c) g8[c] += __ldg(bw.g_feat + si * 20 + c);
+    }
+    if constexpr (DET) {
+        float4* r = reinterpret_cast<float4*>(det.rec + si * 8);
+        r[0] = make_float4(g8[0], g8[1], g8[2], g8[3]);
+        r[1] = make_float4(g8[4], g8[5], g8[6], g8[7]);
+        float m = 0.f;
+        unsigned nonfinite = 0u;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const float a = fabsf(g8[c]);
+            if (a <= FLT_MAX) m = fmaxf(m, a); else nonfinite = 1u;
+        }
+        const unsigned mask = __activemask();
+        const unsigned mb = __reduce_max_sync(mask, __float_as_uint(m)), nf = __reduce_or_sync(mask, nonfinite);
+        if ((tid & 31) == __ffs(mask) - 1) {
+            if (mb) atomicMax(det.amax, mb);
+            if (nf) atomicOr(det.amax + 1, nf);
+        }
+        return;
     }
     const Trilinear t = trilinear_corners(sc, __ldg(io.ndc + si * 3), __ldg(io.ndc + si * 3 + 1), __ldg(io.ndc + si * 3 + 2));
     const int W = sc.Wp, H = sc.Hp, D = sc.D;
@@ -267,8 +308,9 @@ __device__ __forceinline__ void volume_scatter(const SceneDev& sc, const RenderI
     }
 }
 
+template <bool DET>
 __global__ void __launch_bounds__(256, 1)
-render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts) {
+render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts, const DetIO det) {
     extern __shared__ __align__(16) float smem[];
     const TileSmem sm(smem);                       // backward: sm.pe holds peT as [64][H_LD]; sm.h, sm.mod the A operands
     float* s_T    = sm.tail;                       // [128] transmittance in front of the sample
@@ -303,7 +345,7 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
         __syncthreads();
 
         // =============================== compositing: forward + reverse scan ===========================
-        composite_scan(sc, bw, sm, s_T, s_g, grp, R, S, N, tid);
+        composite_scan<DET>(sc, bw, sm, s_T, s_g, grp, R, S, N, tid, det);
         stage_T(sm.pe, scr + bwd::S_PET, 64, tid);             // peT -> shared (used by the layer-5 and layer-0 wgrads)
         __syncthreads();
 
@@ -445,7 +487,7 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
                     *reinterpret_cast<float4*>(s_df + frag_row(ty, r) * 8 + tx * 4) = make_float4(a[r][0], a[r][1], a[r][2], a[r][3]);
             }
             __syncthreads();
-            if (tid < TILE_M && valid) volume_scatter(sc, io, bw, s_df, si, tid);   // trilinear scatter
+            if (tid < TILE_M && valid) volume_scatter<DET>(sc, io, bw, s_df, si, tid, det);   // trilinear scatter
         }
         __syncthreads();
     }
@@ -697,9 +739,10 @@ __device__ __forceinline__ void frag_load_rm(float (&acc)[8][8], const float* sr
     __syncthreads();
 }
 
+template <bool DET>
 __global__ void __launch_bounds__(256, 1)
 render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts,
-                     const __half* __restrict__ wh) {
+                     const __half* __restrict__ wh, const DetIO det) {
     using namespace bwdtc;
     extern __shared__ __align__(16) float smem[];
     const TileSmem sm(smem);
@@ -740,7 +783,7 @@ render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const
         __syncthreads();
         tile_mlp(sm, wts, tid, ScratchRecord{scr});
         __syncthreads();
-        composite_scan(sc, bw, sm, s_T, s_g, grp, R, S, N, tid);
+        composite_scan<DET>(sc, bw, sm, s_T, s_g, grp, R, S, N, tid, det);
         load_w_issue(wh + W_VF, 64 * 128, w16, tid);
         __syncthreads();
         const int e_pe = stage_half(scr + bwd::S_PET, 128, 64, 128, pe16, s_amax, amax_i, tid);
@@ -884,7 +927,7 @@ render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const
                 *reinterpret_cast<float2*>(s_df + (64 * wg + 16 * w + g + 8 * hh) * 8 + 2 * q) =
                     make_float2(d1[0][2 * hh] * sc_m, d1[0][2 * hh + 1] * sc_m);
             __syncthreads();
-            if (tid < TILE_M && valid) volume_scatter(sc, io, bw, s_df, si, tid);
+            if (tid < TILE_M && valid) volume_scatter<DET>(sc, io, bw, s_df, si, tid, det);
         }
         __syncthreads();
     }
@@ -945,6 +988,79 @@ __global__ void adam_volume_cl_kernel(float4* __restrict__ p, float4* __restrict
     }
 }
 
+// ============================== deterministic volume gradient and loss (DET = true) ==============================
+// The float-atomic scatter sums each voxel channel's contributions in whatever order the CTAs reach it.  Here the
+// backward kernel records each sample's 8 gradients g (volume_scatter<true>) and the max |g| over them, and the
+// scatter happens afterwards in integers, which add associatively:
+//   det_scatter_kernel  every contribution g * wgt, formed in fp32 exactly as the atomic path forms it, is scaled by
+//                       2^e and rounded to int64 (red.global.add.u64 into a zeroed [D,Hp,Wp,8] accumulator).  A channel
+//                       receives at most n = N*S contributions (a sample's 8 corners are distinct voxels), each of
+//                       magnitude <= max|g| < 2^(em+1), so e = 61 - ceil(log2 n) - em keeps every partial sum within
+//                       2^62.  Contributions below half a quantum 2^-e (~ max|g| * n * 2^-62) round to zero.
+//                       A non-finite contribution is added as a float to the fp32 gradient itself, so the entries it
+//                       touches become NaN / inf as with the float atomics (and in any order).
+//   det_convert_kernel  grad += float(acc) * 2^-e: one correctly rounded conversion, then an exact power-of-two scale.
+//   loss_reduce_kernel  the per-ray loss terms in a fixed order (one block, fp64 partial sums) -> += loss_out.
+// With max|g| == 0 nothing is scattered or converted (the accumulator stays zero).
+__device__ __forceinline__ int det_scale_exp(unsigned amax_bits, long long n) {
+    const int em = (int)(amax_bits >> 23) - 127;               // max|g| < 2^(em+1); a subnormal max gives em = -127
+    const int k = 64 - __clzll(n - 1);                          // n <= 2^k
+    return 61 - k - em;                                         // -106 <= e <= 188 for n <= 2^40: a double scale
+}
+
+__global__ void det_scatter_kernel(const SceneDev sc, const float* __restrict__ ndc, const float* __restrict__ rec,
+                                   const unsigned* __restrict__ amax, long long nsamp,
+                                   unsigned long long* __restrict__ acc, float* __restrict__ dvol) {
+    const unsigned mb = amax[0];
+    if (mb == 0u && amax[1] == 0u) return;                      // all-zero gradients
+    const double s = __longlong_as_double((long long)(1023 + det_scale_exp(mb, nsamp)) << 52);
+    const int W = sc.Wp, H = sc.Hp, D = sc.D;
+    // thread t: sample t >> 6, corner (t >> 3) & 7, channel t & 7 -- a warp adds 4 corners x 64 contiguous bytes
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < nsamp * 64; t += (long long)gridDim.x * blockDim.x) {
+        const long long si = t >> 6;
+        const int c = (int)(t >> 3) & 7, ch = (int)t & 7;
+        const float g = __ldg(rec + si * 8 + ch);
+        if (g == 0.f) continue;
+        const Trilinear tr = trilinear_corners(sc, __ldg(ndc + si * 3), __ldg(ndc + si * 3 + 1), __ldg(ndc + si * 3 + 2));
+        const int x = tr.x0 + (c & 1), y = tr.y0 + ((c >> 1) & 1), z = tr.z0 + (c >> 2);
+        if ((unsigned)x >= (unsigned)W || (unsigned)y >= (unsigned)H || (unsigned)z >= (unsigned)D) continue;   // zeros padding
+        const float wgt = tr.wx[c & 1] * tr.wy[(c >> 1) & 1] * tr.wz[c >> 2];
+        const float p = g * wgt;
+        const size_t o = (((size_t)z * H + y) * W + x) * 8 + ch;
+        if (!(fabsf(p) <= FLT_MAX)) { atomicAdd(dvol + o, p); continue; }
+        const long long q = __double2ll_rn((double)p * s);
+        if (q != 0) asm volatile("red.global.add.u64 [%0], %1;" ::"l"(acc + o), "l"(q) : "memory");
+    }
+}
+
+__global__ void det_convert_kernel(const longlong2* __restrict__ acc, const unsigned* __restrict__ amax, long long nsamp,
+                                   float2* __restrict__ dvol, long long n2) {
+    const unsigned mb = amax[0];
+    if (mb == 0u) return;
+    const int e = det_scale_exp(mb, nsamp);
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n2; i += (long long)gridDim.x * blockDim.x) {
+        const longlong2 a = acc[i];
+        if ((a.x | a.y) == 0) continue;                         // untouched (or exactly cancelled): the gradient is as it was
+        float2 d = dvol[i];
+        if (a.x) d.x += ldexpf(__ll2float_rn(a.x), -e);
+        if (a.y) d.y += ldexpf(__ll2float_rn(a.y), -e);
+        dvol[i] = d;
+    }
+}
+
+__global__ void __launch_bounds__(1024) loss_reduce_kernel(const float* __restrict__ terms, int n, float* __restrict__ loss) {
+    __shared__ double part[1024];
+    double a = 0.0;
+    for (int i = threadIdx.x; i < n; i += 1024) a += (double)terms[i];
+    part[threadIdx.x] = a;
+    __syncthreads();
+    for (int w = 512; w > 0; w >>= 1) {
+        if ((int)threadIdx.x < w) part[threadIdx.x] += part[threadIdx.x + w];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *loss += (float)part[0];
+}
+
 static int bwd_grid(int N, int S) {
     const int R = TILE_M / S;
     const int ngroups = (N + R - 1) / R;
@@ -965,23 +1081,65 @@ size_t render_backward_tc_workspace_bytes(int N, int S) {
     return ctas * (bwd::SCRATCH + bwd::GRADS) * sizeof(float) + bwdtc::WIMG * sizeof(__half);
 }
 
+// Deterministic variant: the workspace of the grad mode, then (256-byte aligned) the [N] loss terms, and with a volume
+// gradient the two amax words (in a 256-byte slot), the int64 accumulator [D,Hp,Wp,8] right behind them (one memset
+// zeroes both) and the [N*S][8] record.
+namespace {
+struct DetLayout { size_t loss, amax, acc, rec, total; };
+DetLayout det_layout(size_t base, int N, int S, size_t nvox) {
+    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    DetLayout l{};
+    l.loss = up(base);
+    l.amax = up(l.loss + (size_t)N * sizeof(float));
+    l.acc = l.amax + 256;
+    l.rec = up(l.acc + nvox * 8 * sizeof(long long));
+    l.total = nvox ? l.rec + (size_t)N * S * 8 * sizeof(float) : l.amax;
+    return l;
+}
+}  // namespace
+
+size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc) {
+    const bool frozen = D == 0 && Hp == 0 && Wp == 0;
+    if (!frozen && (D <= 0 || Hp <= 0 || Wp <= 0)) return 0;
+    const size_t base = tc ? render_backward_tc_workspace_bytes(N, S) : render_backward_workspace_bytes(N, S);
+    if (base == 0) return 0;
+    return det_layout(base, N, S, (size_t)D * Hp * Wp).total;
+}
+
 int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const float* const* mlp_w,
                            const float* g_rgb, const float* target, float inv_count, const float* g_depth,
                            const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
                            float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream, bool tc) {
-    const char* what = tc ? "render backward (grad_mode TC_HALF)" : "render backward";
+                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det) {
+    const char* what = det ? (tc ? "deterministic render backward (grad_mode TC_HALF)" : "deterministic render backward")
+                           : (tc ? "render backward (grad_mode TC_HALF)" : "render backward");
     MVSN_REQUIRE(io.S <= TILE_M, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, io.S);
-    const size_t need = tc ? render_backward_tc_workspace_bytes(io.N, io.S) : render_backward_workspace_bytes(io.N, io.S);
+    const size_t base = tc ? render_backward_tc_workspace_bytes(io.N, io.S) : render_backward_workspace_bytes(io.N, io.S);
+    const size_t nvox = dvol ? (size_t)sc.D * sc.Hp * sc.Wp : 0;
+    const DetLayout dl = det_layout(base, io.N, io.S, nvox);
+    const size_t need = det ? dl.total : base;
     MVSN_REQUIRE(workspace && workspace_bytes >= need, MVSN_EWORKSPACE, "%s: workspace %zu < %zu bytes", what, workspace_bytes, need);
     MVSN_REQUIRE(aligned16(workspace), MVSN_EALIGN, "%s: workspace must be 16-byte aligned", what);
-    static bool attr_set[2][64] = {};
+    static bool attr_set[4][64] = {};
+    const int kind = (tc ? 2 : 0) + (det ? 1 : 0);
     int dev = 0;
     MVSN_CUDA_CHECK(cudaGetDevice(&dev));
-    if (dev >= 64 || !attr_set[tc][dev]) {
-        if (tc) MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
-        else    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
-        if (dev < 64) attr_set[tc][dev] = true;
+    if (dev >= 64 || !attr_set[kind][dev]) {
+        const void* kfn = tc ? (det ? (const void*)render_bwd_tc_kernel<true> : (const void*)render_bwd_tc_kernel<false>)
+                             : (det ? (const void*)render_bwd_kernel<true> : (const void*)render_bwd_kernel<false>);
+        MVSN_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+        if (dev < 64) attr_set[kind][dev] = true;
+    }
+    DetIO dt{};
+    if (det) {
+        char* w8 = static_cast<char*>(workspace);
+        dt.loss_terms = reinterpret_cast<float*>(w8 + dl.loss);
+        if (dvol) {
+            dt.amax = reinterpret_cast<unsigned*>(w8 + dl.amax);
+            dt.rec = reinterpret_cast<float*>(w8 + dl.rec);
+            // the workspace is shared between modes and callers may hand it over uninitialised: zero every call
+            MVSN_CUDA_CHECK(cudaMemsetAsync(w8 + dl.amax, 0, dl.rec - dl.amax, stream));
+        }
     }
     const int grid = bwd_grid(io.N, io.S);
     float* ws = static_cast<float*>(workspace);
@@ -997,18 +1155,36 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
         __half* wh = reinterpret_cast<__half*>(wimg);
         pack_dgrad_half_kernel<<<64, 256, 0, stream>>>(wp, wh);
         MVSN_CUDA_CHECK(cudaGetLastError());
-        render_bwd_tc_kernel<<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, wh);
+        if (det) render_bwd_tc_kernel<true><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, wh, dt);
+        else     render_bwd_tc_kernel<false><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, wh, dt);
     } else {
         bw.wd = wimg;
         pack_dgrad_kernel<<<64, 256, 0, stream>>>(wp, wimg);
         MVSN_CUDA_CHECK(cudaGetLastError());
-        render_bwd_kernel<<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32);
+        if (det) render_bwd_kernel<true><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, dt);
+        else     render_bwd_kernel<false><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, dt);
     }
     MVSN_CUDA_CHECK(cudaGetLastError());
     GradOut go;
     for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) go.p[i] = grad_mlp[i];
     mlp_grad_reduce_kernel<<<dim3(16, MVSN_N_MLP_TENSORS), 256, 0, stream>>>(bw.grads, grid, go);
     MVSN_CUDA_CHECK(cudaGetLastError());
+    if (det && dvol) {
+        const long long nsamp = (long long)io.N * io.S;
+        auto* acc = reinterpret_cast<unsigned long long*>(static_cast<char*>(workspace) + dl.acc);
+        const int gs = cdiv(nsamp * 64, 256) < sm_count() * 16 ? cdiv(nsamp * 64, 256) : sm_count() * 16;
+        det_scatter_kernel<<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, dvol);
+        MVSN_CUDA_CHECK(cudaGetLastError());
+        const long long n2 = (long long)nvox * 4;               // (int64 pair, float pair) per thread step
+        const int gc = cdiv(n2, 256) < sm_count() * 8 ? cdiv(n2, 256) : sm_count() * 8;
+        det_convert_kernel<<<gc, 256, 0, stream>>>(reinterpret_cast<const longlong2*>(acc), dt.amax, nsamp,
+                                                   reinterpret_cast<float2*>(dvol), n2);
+        MVSN_CUDA_CHECK(cudaGetLastError());
+    }
+    if (det && loss && target) {                                // the terms exist only with the fused loss
+        loss_reduce_kernel<<<1, 1024, 0, stream>>>(dt.loss_terms, io.N, loss);
+        MVSN_CUDA_CHECK(cudaGetLastError());
+    }
     return MVSN_OK;
 }
 

@@ -68,14 +68,16 @@ int launch_render_fp32(const SceneDev& sc, const RenderIO& io, bool fast, const 
 int launch_render_wg(const SceneDev& sc, const RenderIO& io, bool fast, bool split, const void* wimg, cudaStream_t stream);
 size_t mlp_wg_packed_bytes(bool split);
 int pack_mlp_wg(const float* const* w, bool split, void* packed, cudaStream_t stream);
-// fine-tuning step (render_bwd.cu); tc: dgrad / wgrad GEMMs on wgmma with fp16 operands (grad_mode TC_HALF)
+// fine-tuning step (render_bwd.cu); tc: dgrad / wgrad GEMMs on wgmma with fp16 operands (grad_mode TC_HALF);
+// det: the volume gradient and the loss summed in a fixed order (bit-reproducible)
 size_t render_backward_workspace_bytes(int N, int S);
 size_t render_backward_tc_workspace_bytes(int N, int S);
+size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc);
 int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const float* const* mlp_w,
                            const float* g_rgb, const float* target, float inv_count, const float* g_depth,
                            const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
                            float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream, bool tc);
+                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det);
 int launch_adam_tensors(float* const* p, const float* const* g, float* const* m, float* const* v, const int* n, int count,
                         float lr, float beta1, float beta2, float eps, int step, cudaStream_t stream);
 int launch_adam_volume(float* p, float* g_dhwc, float* m, float* v, long long nvox, int planar, float lr, float beta1,
