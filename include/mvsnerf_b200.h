@@ -200,6 +200,26 @@ int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const flo
                                        const float* rays_dir, int N, int S, int grad_mode, const mvsn_render_grads* g,
                                        float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
                                        size_t workspace_bytes, void* stream);
+/* mvsn_render_backward_rays: the fine-tuning step straight from rays, as train_mvs_nerf_finetuning_pl.py:140-164 feeds
+ * it -- the backward kernel also replaces data/ray_utils.ray_marcher (with perturb) and utils.get_ndc_coordinate, so
+ * no per-sample array is read.  rays [N,8], t_steps [S] and rp as mvsn_render_rays (rays 16-byte aligned);
+ * jitter [N,S] = perturb * u, u uniform in [0,1) as the caller's RNG draws it (NULL: no jitter, the depths are exactly
+ * mvsn_render_rays'): sample s of a ray lies at lower + (upper - lower) * jitter, between the midpoints of the
+ * neighbouring unjittered depths (data/ray_utils.py:184-191), each operation rounded as fp32 element-wise ops round it.
+ * grad_mode MVSN_MLP_FP32 or MVSN_MLP_TC_HALF selects the arithmetic of the GEMMs as mvsn_render_backward /
+ * mvsn_render_backward_tc do; deterministic != 0 sums the volume gradient and the loss as
+ * mvsn_render_backward_deterministic does.  g, grad_mlp and grad_volume_dhwc as mvsn_render_backward; rgb_out /
+ * depth_out receive the forward of the marched samples (with jitter = NULL: rgb bit-identical to mvsn_render_rays with
+ * the MVSN_MLP_FP32 image).  N_samples <= 128.  Argument errors are returned before any CUDA call: an unknown grad_mode
+ * (MVSN_EUNSUPPORTED) first, then NULL pointers, a misaligned rays, then N_samples > 128 (MVSN_EUNSUPPORTED).
+ * Workspace: mvsn_render_backward_rays_workspace_bytes(N, S, D, Hp, Wp, grad_mode, deterministic) bytes, 16-byte
+ * aligned; the volume dims matter only with `deterministic` (D = Hp = Wp = 0: a frozen volume).  0 for an unknown
+ * grad_mode or shape. */
+size_t mvsn_render_backward_rays_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic);
+int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
+                              const float* rays, const float* t_steps, const float* jitter, int N, int S, int grad_mode,
+                              int deterministic, const mvsn_render_grads* g, float* const* grad_mlp,
+                              float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream);
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
                    const int* numel_host, int count, float lr, float beta1, float beta2, float eps, int step,
                    void* stream);

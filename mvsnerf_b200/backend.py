@@ -660,6 +660,32 @@ def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_featu
         grad_mlp = [torch.empty_like(p) for p in params]
     if want_volume_grad and grad_volume is None:
         grad_volume = torch.zeros(sc.D, sc.Hp, sc.Wp, 8, dtype=torch.float32, device=dev)
+    g, held, rgb, depth = _render_grads(N, S, dev, grads, target_rgb, n_total, want_forward, loss_out)
+    vol_arg = _lib.ptr(grad_volume) if want_volume_grad else None
+    if torch.are_deterministic_algorithms_enabled():
+        ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode, (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0))
+        with torch.cuda.device(dev):
+            _lib.check(lib.mvsn_render_backward_deterministic(
+                C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z), _lib.ptr(dirs), N, S,
+                int(grad_mode), C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(ws), ws_bytes,
+                _lib.stream_ptr()), "mvsn_render_backward_deterministic")
+        del keep, held
+        return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
+    ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode)
+    entry, name = ((lib.mvsn_render_backward_tc, "mvsn_render_backward_tc") if grad_mode == _lib.MLP_TC_HALF
+                   else (lib.mvsn_render_backward, "mvsn_render_backward"))
+    with torch.cuda.device(dev):
+        _lib.check(entry(C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z),
+                         _lib.ptr(dirs), N, S, C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(ws), ws_bytes,
+                         _lib.stream_ptr()), name)
+    del keep, held
+    return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
+
+
+def _render_grads(N, S, dev, grads, target_rgb, n_total, want_forward, loss_out):
+    """The lib.RenderGrads of a backward launch over N rays x S samples: the cotangents (`grads`) or the fused loss
+    (`target_rgb`, normalised by 3 * n_total), and the optional forward / loss outputs.  Returns (g, the device tensors
+    g points into, rgb [N,3] or None, depth [N] or None)."""
     g = _lib.RenderGrads()
     held = []
 
@@ -691,23 +717,59 @@ def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_featu
         g.rgb_out, g.depth_out = rgb.data_ptr(), depth.data_ptr()
     if loss_out is not None:
         g.loss_out = loss_out.data_ptr()
-    vol_arg = _lib.ptr(grad_volume) if want_volume_grad else None
-    if torch.are_deterministic_algorithms_enabled():
-        ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode, (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0))
-        with torch.cuda.device(dev):
-            _lib.check(lib.mvsn_render_backward_deterministic(
-                C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z), _lib.ptr(dirs), N, S,
-                int(grad_mode), C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(ws), ws_bytes,
-                _lib.stream_ptr()), "mvsn_render_backward_deterministic")
-        del keep, held
-        return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
-    ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode)
-    entry, name = ((lib.mvsn_render_backward_tc, "mvsn_render_backward_tc") if grad_mode == _lib.MLP_TC_HALF
-                   else (lib.mvsn_render_backward, "mvsn_render_backward"))
+    return g, held, rgb, depth
+
+
+def _tsteps_of(S, dev):
+    """torch.linspace(0, 1, S) on `dev` (data/ray_utils.py:175), cached: the t_steps of the in-kernel ray march."""
+    tk = (S, dev)
+    if tk not in _tsteps:
+        _tsteps[tk] = torch.linspace(0, 1, S, device=dev)
+    return _tsteps[tk]
+
+
+def render_backward_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad, N_samples=128, lindisp=False,
+                         jitter=None, white_bkgd=False, grads=None, target_rgb=None, n_total=None, want_volume_grad=True,
+                         grad_volume=None, grad_mlp=None, want_forward=False, loss_out=None, grad_mode=_lib.MLP_FP32):
+    """render_backward straight from rays [N,8] = (o, d, near, far): one mvsn_render_backward_rays launch, whose kernel
+    also does ray_marcher and get_ndc_coordinate (data/ray_utils.py:152-197, utils.py:112-146) for the reference camera.
+    `near_far` / `pad` / `N_samples` / `lindisp` as in render_rays.  `jitter` [N, N_samples] = perturb * u, the uniform
+    draw ray_marcher makes with perturb > 0: sample s then lies at lower + (upper - lower) * jitter between the
+    midpoints of its neighbours' depths, rounded as ray_marcher rounds it; None marches exactly render_rays' depths.
+    Everything else, the return value and the grad_mode / torch.use_deterministic_algorithms dispatch are as in
+    render_backward (the depth the `grads` dict differentiates is the jittered one)."""
+    _check_grad_mode(grad_mode)
+    lib = _lib.load()
+    rays = _lib.dev_f32(rays.detach(), "rays")
+    N, S = rays.shape[0], int(N_samples)
+    dev = rays.device
+    if jitter is not None:
+        jitter = _lib.dev_f32(jitter.detach(), "jitter")
+        if tuple(jitter.shape) != (N, S):
+            raise RuntimeError(f"render_backward_rays: jitter must be [{N}, {S}], got {tuple(jitter.shape)}")
+    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, _lib.MLP_FP32)
+    rp = _lib.RayParams(float(near_far[0]), float(near_far[1]), float(pad), int(bool(lindisp)))
+    params = [_lib.dev_f32(p.detach(), "MLP parameter") for p in network_fn.ordered_params()]
+    if grad_mlp is None:
+        grad_mlp = [torch.empty_like(p) for p in params]
+    if want_volume_grad and grad_volume is None:
+        grad_volume = torch.zeros(sc.D, sc.Hp, sc.Wp, 8, dtype=torch.float32, device=dev)
+    g, held, rgb, depth = _render_grads(N, S, dev, grads, target_rgb, n_total, want_forward, loss_out)
+    det = torch.are_deterministic_algorithms_enabled()
+    dims = (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0)
+    need = lib.mvsn_render_backward_rays_workspace_bytes(N, S, *dims, int(grad_mode), int(det))
+    if need == 0:
+        raise RuntimeError(f"render_backward_rays: unsupported shape N={N}, N_samples={S} (N_samples <= 128)")
+    ws = _bwd_workspace.get(dev)
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        _bwd_workspace[dev] = ws
     with torch.cuda.device(dev):
-        _lib.check(entry(C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z),
-                         _lib.ptr(dirs), N, S, C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(ws), ws_bytes,
-                         _lib.stream_ptr()), name)
+        _lib.check(lib.mvsn_render_backward_rays(
+            C.byref(sc), _lib.ptr_array(params), C.byref(rp), _lib.ptr(rays), _lib.ptr(_tsteps_of(S, dev)),
+            _lib.ptr(jitter), N, S, int(grad_mode), int(det), C.byref(g), _lib.ptr_array(grad_mlp),
+            _lib.ptr(grad_volume) if want_volume_grad else None, _lib.ptr(ws), need, _lib.stream_ptr()),
+            "mvsn_render_backward_rays")
     del keep, held
     return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
 
@@ -723,7 +785,8 @@ class FineTuner:
     render entry points and scene_io see them as after a torch.optim.Adam step with the same hyper-parameters.
     grad_mode=MLP_TC_HALF runs the backward's dgrad / wgrad GEMMs on tensor cores (see render_backward).  Under
     torch.use_deterministic_algorithms(True) every step is bit-reproducible: two runs from the same start on the same
-    batches end with identical parameters, volume and losses (see render_backward)."""
+    batches end with identical parameters, volume and losses (see render_backward).  `step` takes marched samples;
+    `step_rays` takes the rays and marches them inside the backward kernel (three launches)."""
 
     def __init__(self, network_fn, volume, imgs, pose_ref, lr=5e-4, betas=(0.9, 0.999), eps=1e-8, white_bkgd=False,
                  grad_mode=_lib.MLP_FP32):
@@ -758,7 +821,6 @@ class FineTuner:
     def step(self, rays_pts, rays_ndc, z_vals, rays_dir, target_rgb, lr=None, want_forward=False):
         """One optimisation step on a batch.  Returns (loss [1] device tensor -- img2mse of this batch BEFORE the
         update, as the reference logs it -- and (rgb, depth) of the forward pass when `want_forward`)."""
-        lib = _lib.load()
         lr = self.lr if lr is None else float(lr)
         self.step_count += 1
         self.loss.zero_()
@@ -766,6 +828,35 @@ class FineTuner:
                                            self.network_fn, self.white_bkgd, target_rgb=target_rgb, want_volume_grad=True,
                                            grad_volume=self.vol_g, grad_mlp=self.g, want_forward=want_forward,
                                            loss_out=self.loss, grad_mode=self.grad_mode)
+        self._adam(lr)
+        return self.loss, (rgb, depth)
+
+    def step_rays(self, rays, target_rgb, near_far, pad, N_samples=128, lindisp=False, perturb=1.0, generator=None,
+                  lr=None, want_forward=False):
+        """One optimisation step on a batch of rays [N,8] = (o, d, near, far), as train_mvs_nerf_finetuning_pl.py:140-164
+        feeds it: the ray march (ray_marcher with `perturb`) and the NDC conversion run inside the backward kernel
+        (render_backward_rays).  With perturb > 0 the jitter is drawn as ray_marcher draws it, `perturb *
+        torch.rand((N, N_samples))` (from `generator`, or the default generator), so switching a run from
+        `step(*ray_marcher(...))` to step_rays consumes the same random stream.  `near_far` / `pad` as in render_rays.
+        Returns what `step` returns."""
+        lr = self.lr if lr is None else float(lr)
+        rays = _lib.dev_f32(rays.detach(), "rays")
+        jitter = None
+        if perturb > 0:
+            jitter = perturb * torch.rand((rays.shape[0], int(N_samples)), device=rays.device, generator=generator)
+        self.step_count += 1
+        self.loss.zero_()
+        _, _, rgb, depth = render_backward_rays(rays, self.volume, self.imgs, self.pose_ref, self.network_fn, near_far,
+                                                pad, N_samples=N_samples, lindisp=lindisp, jitter=jitter,
+                                                white_bkgd=self.white_bkgd, target_rgb=target_rgb, want_volume_grad=True,
+                                                grad_volume=self.vol_g, grad_mlp=self.g, want_forward=want_forward,
+                                                loss_out=self.loss, grad_mode=self.grad_mode)
+        self._adam(lr)
+        return self.loss, (rgb, depth)
+
+    def _adam(self, lr):
+        """mvsn_adam_step + mvsn_adam_step_volume on the gradients of the step's backward launch."""
+        lib = _lib.load()
         dev = self.params[0].device
         fv = self.volume.feat_volume
         with torch.cuda.device(dev):
@@ -779,7 +870,6 @@ class FineTuner:
                        "mvsn_adam_step_volume")
         # the parameters changed behind PyTorch's back: bump their version counters (weight-image / volume caches)
         torch.autograd.graph.increment_version([p for p in self.params] + [fv])
-        return self.loss, (rgb, depth)
 
 
 def ray_marcher(rays, N_samples=64, lindisp=False, perturb=0):
@@ -915,9 +1005,7 @@ def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
     N = rays.shape[0]
     dev = rays.device
     S = int(N_samples)
-    tk = (S, dev)
-    if tk not in _tsteps:
-        _tsteps[tk] = torch.linspace(0, 1, S, device=dev)          # data/ray_utils.py:175
+    t_steps = _tsteps_of(S, dev)
     sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode)
     rp = _lib.RayParams(float(near_far[0]), float(near_far[1]), float(pad), int(bool(lindisp)))
     if out is not None:
@@ -929,11 +1017,11 @@ def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
         depth = torch.empty(N, dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
         if sink is not None:
-            _lib.check(lib.mvsn_render_rays_to_peers(C.byref(sc), C.byref(rp), _lib.ptr(rays), _lib.ptr(_tsteps[tk]), N, S,
+            _lib.check(lib.mvsn_render_rays_to_peers(C.byref(sc), C.byref(rp), _lib.ptr(rays), _lib.ptr(t_steps), N, S,
                                                      C.byref(sink), _lib.ptr(rgb), _lib.ptr(depth), _lib.stream_ptr()),
                        "mvsn_render_rays_to_peers")
         else:
-            _lib.check(lib.mvsn_render_rays(C.byref(sc), C.byref(rp), _lib.ptr(rays), _lib.ptr(_tsteps[tk]), N, S,
+            _lib.check(lib.mvsn_render_rays(C.byref(sc), C.byref(rp), _lib.ptr(rays), _lib.ptr(t_steps), N, S,
                                             _lib.ptr(rgb), _lib.ptr(depth), None, None, None, _lib.stream_ptr()),
                        "mvsn_render_rays")
     del keep

@@ -240,6 +240,20 @@ int mvsn_render_samples(const mvsn_render_scene* scene, const float* rays_pts, c
     return dispatch_render(scene, sc, io, false, (cudaStream_t)stream);
 }
 
+// host-side scalars of the in-kernel ray march exactly as utils.get_ndc_coordinate forms them (python floats -> fp32)
+static RayGenDev make_ray_gen(const mvsn_render_scene* scene, const mvsn_ray_params* rp) {
+    RayGenDev rg;
+    rg.near = rp->ndc_near;
+    rg.far_minus_near = (float)((double)rp->ndc_far - (double)rp->ndc_near);
+    rg.inv_near = (float)(1.0 / (double)rp->ndc_near);
+    rg.inv_far_minus_inv_near = (float)(1.0 / (double)rp->ndc_far - 1.0 / (double)rp->ndc_near);
+    rg.pad = rp->pad;
+    rg.wf = (float)scene->W / 4.0f;     // (inv_scale + 1) / 4, utils.py:139
+    rg.hf = (float)scene->H / 4.0f;
+    rg.lindisp = rp->lindisp;
+    return rg;
+}
+
 static int render_rays_impl(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const float* rays,
                             const float* t_steps, int N, int S, float* rgb, float* depth, float* weights,
                             float* alpha, float* input_feat, const mvsn_peer_sink* sink, void* stream) {
@@ -257,15 +271,7 @@ static int render_rays_impl(const mvsn_render_scene* scene, const mvsn_ray_param
     io.rays = rays; io.t_steps = t_steps;
     io.N = N; io.S = S;
     io.rgb = rgb; io.depth = depth; io.weights = weights; io.alpha = alpha; io.input_feat = input_feat;
-    // host-side scalars exactly as utils.get_ndc_coordinate forms them (python floats -> fp32)
-    io.rg.near = rp->ndc_near;
-    io.rg.far_minus_near = (float)((double)rp->ndc_far - (double)rp->ndc_near);
-    io.rg.inv_near = (float)(1.0 / (double)rp->ndc_near);
-    io.rg.inv_far_minus_inv_near = (float)(1.0 / (double)rp->ndc_far - 1.0 / (double)rp->ndc_near);
-    io.rg.pad = rp->pad;
-    io.rg.wf = (float)scene->W / 4.0f;     // (inv_scale + 1) / 4, utils.py:139
-    io.rg.hf = (float)scene->H / 4.0f;
-    io.rg.lindisp = rp->lindisp;
+    io.rg = make_ray_gen(scene, rp);
     if (sink) {
         MVSN_REQUIRE(sink->n_peers >= 1 && sink->n_peers <= MVSN_MAX_PEERS, MVSN_EBADSHAPE,
                      "peer sink: n_peers=%d (1..%d)", sink->n_peers, MVSN_MAX_PEERS);
@@ -367,6 +373,45 @@ int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const flo
                  "mvsn_render_backward_deterministic: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)", grad_mode);
     return render_backward_entry(scene, mlp_w, rays_pts, rays_ndc, z_vals, rays_dir, N, S, g, grad_mlp, grad_volume_dhwc,
                                  workspace, workspace_bytes, stream, grad_mode == MVSN_MLP_TC_HALF, true);
+}
+
+size_t mvsn_render_backward_rays_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
+    if (grad_mode != MVSN_MLP_FP32 && grad_mode != MVSN_MLP_TC_HALF) return 0;
+    const bool tc = grad_mode == MVSN_MLP_TC_HALF;
+    if (deterministic) return render_backward_det_workspace_bytes(N, S, D, Hp, Wp, tc);
+    return tc ? render_backward_tc_workspace_bytes(N, S) : render_backward_workspace_bytes(N, S);
+}
+
+int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
+                              const float* rays, const float* t_steps, const float* jitter, int N, int S, int grad_mode,
+                              int deterministic, const mvsn_render_grads* g, float* const* grad_mlp,
+                              float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward_rays");
+    MVSN_REQUIRE(grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF, MVSN_EUNSUPPORTED,
+                 "mvsn_render_backward_rays: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)", grad_mode);
+    SceneDev sc;
+    int rc = make_scene(scene, sc);
+    if (rc) return rc;
+    MVSN_REQUIRE(rp && g && mlp_w && grad_mlp, MVSN_ENULL, "mvsn_render_backward_rays: NULL argument");
+    MVSN_REQUIRE(g->rgb || g->target_rgb, MVSN_ENULL, "mvsn_render_backward_rays: neither g->rgb nor g->target_rgb given");
+    for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i)
+        MVSN_REQUIRE(mlp_w[i] && grad_mlp[i], MVSN_ENULL, "mvsn_render_backward_rays: tensor %d is NULL", i);
+    MVSN_REQUIRE(N == 0 || (rays && t_steps), MVSN_ENULL, "mvsn_render_backward_rays: rays or t_steps is NULL");
+    MVSN_REQUIRE(aligned16(rays), MVSN_EALIGN, "mvsn_render_backward_rays: rays must be 16-byte aligned");
+    MVSN_REQUIRE(!grad_volume_dhwc || aligned16(grad_volume_dhwc), MVSN_EALIGN, "grad_volume_dhwc must be 16-byte aligned");
+    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "mvsn_render_backward_rays: N=%d S=%d", N, S);
+    MVSN_REQUIRE(S <= 128, MVSN_EUNSUPPORTED, "mvsn_render_backward_rays: N_samples=%d > 128 is not implemented", S);
+    MVSN_REQUIRE(scene->mlp_mode == MVSN_MLP_FP32, MVSN_EUNSUPPORTED,
+                 "mvsn_render_backward_rays: scene->mlp_packed must be the MVSN_MLP_FP32 image (mode %d given)", scene->mlp_mode);
+    if (N == 0) return MVSN_OK;
+    RenderIO io{};
+    io.rays = rays; io.t_steps = t_steps;
+    io.rg = make_ray_gen(scene, rp);
+    io.N = N; io.S = S;
+    return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
+                                  g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
+                                  grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
+                                  (cudaStream_t)stream, grad_mode == MVSN_MLP_TC_HALF, deterministic != 0, jitter);
 }
 
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,

@@ -31,6 +31,10 @@
 // mvsn_render_backward_deterministic runs either kernel with DET = true: the volume scatter and the fused loss are
 // recorded instead of summed with float atomics, then summed in a fixed-point scatter and a fixed-order reduction
 // (described above det_scatter_kernel), so every output is bit-reproducible.
+//
+// mvsn_render_backward_rays runs any of these with FAST = true: the front end marches the samples from the rays, as
+// render_rays does, with stratified depths from a caller-drawn jitter (ray_z_jittered), instead of reading the
+// per-sample arrays of ray_marcher / get_ndc_coordinate.
 #include <cfloat>
 
 #include "tile_fp32.cuh"
@@ -266,9 +270,11 @@ __device__ __forceinline__ void trunk_elementwise(float (&acc)[8][8], float* scr
 // DET: the 8 gradients are recorded to det.rec[si] and folded into det.amax (max |g| over the finite values, as float
 // bits with an integer atomicMax, so the result does not depend on the order; any non-finite value sets amax[1]);
 // det_scatter_kernel scatters them afterwards.  The caller is divergent (valid rows only), hence __activemask.
-template <bool DET>
+// The sample's NDC: io.ndc[si], or (FAST: marched in the kernel) rows 0..2 of the recorded positional encoding peT in the
+// CTA's scratch -- the front end's own values, so the scatter hits exactly the corners the forward sampled.
+template <bool DET, bool FAST>
 __device__ __forceinline__ void volume_scatter(const SceneDev& sc, const RenderIO& io, const BwdIO& bw, const float* s_df,
-                                               size_t si, int tid, const DetIO& det) {
+                                               size_t si, int tid, const DetIO& det, const float* scr) {
     float g8[8];
 #pragma unroll
     for (int c = 0; c < 8; ++c) g8[c] = s_df[tid * 8 + c];
@@ -295,7 +301,9 @@ __device__ __forceinline__ void volume_scatter(const SceneDev& sc, const RenderI
         }
         return;
     }
-    const Trilinear t = trilinear_corners(sc, __ldg(io.ndc + si * 3), __ldg(io.ndc + si * 3 + 1), __ldg(io.ndc + si * 3 + 2));
+    Trilinear t;
+    if constexpr (FAST) t = trilinear_corners(sc, scr[bwd::S_PET + tid], scr[bwd::S_PET + 128 + tid], scr[bwd::S_PET + 256 + tid]);
+    else t = trilinear_corners(sc, __ldg(io.ndc + si * 3), __ldg(io.ndc + si * 3 + 1), __ldg(io.ndc + si * 3 + 2));
     const int W = sc.Wp, H = sc.Hp, D = sc.D;
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
@@ -308,9 +316,12 @@ __device__ __forceinline__ void volume_scatter(const SceneDev& sc, const RenderI
     }
 }
 
-template <bool DET>
+// FAST: the front end marches the samples from io.rays / io.t_steps (stratified by `jitter` [N,S] unless NULL) instead of
+// reading io.pts / io.ndc / io.z / io.dirs (mvsn_render_backward_rays); `jitter` is unused otherwise.
+template <bool DET, bool FAST>
 __global__ void __launch_bounds__(256, 1)
-render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts, const DetIO det) {
+render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts, const DetIO det,
+                  const float* __restrict__ jitter) {
     extern __shared__ __align__(16) float smem[];
     const TileSmem sm(smem);                       // backward: sm.pe holds peT as [64][H_LD]; sm.h, sm.mod the A operands
     float* s_T    = sm.tail;                       // [128] transmittance in front of the sample
@@ -338,7 +349,7 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
             const int r_in = tid / S, s_idx = tid - r_in * S, ray = grp * R + r_in;
             valid = r_in < R && ray < N;
             si = (size_t)ray * S + s_idx;
-            tile_front_end<false>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr});
+            tile_front_end<FAST>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr}, jitter);
         }
         __syncthreads();
         tile_mlp(sm, wts, tid, ScratchRecord{scr});
@@ -487,7 +498,7 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
                     *reinterpret_cast<float4*>(s_df + frag_row(ty, r) * 8 + tx * 4) = make_float4(a[r][0], a[r][1], a[r][2], a[r][3]);
             }
             __syncthreads();
-            if (tid < TILE_M && valid) volume_scatter<DET>(sc, io, bw, s_df, si, tid, det);   // trilinear scatter
+            if (tid < TILE_M && valid) volume_scatter<DET, FAST>(sc, io, bw, s_df, si, tid, det, scr);   // trilinear scatter
         }
         __syncthreads();
     }
@@ -739,10 +750,10 @@ __device__ __forceinline__ void frag_load_rm(float (&acc)[8][8], const float* sr
     __syncthreads();
 }
 
-template <bool DET>
+template <bool DET, bool FAST>
 __global__ void __launch_bounds__(256, 1)
 render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts,
-                     const __half* __restrict__ wh, const DetIO det) {
+                     const __half* __restrict__ wh, const DetIO det, const float* __restrict__ jitter) {
     using namespace bwdtc;
     extern __shared__ __align__(16) float smem[];
     const TileSmem sm(smem);
@@ -778,7 +789,7 @@ render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const
             const int r_in = tid / S, s_idx = tid - r_in * S, ray = grp * R + r_in;
             valid = r_in < R && ray < N;
             si = (size_t)ray * S + s_idx;
-            tile_front_end<false>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr});
+            tile_front_end<FAST>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr}, jitter);
         }
         __syncthreads();
         tile_mlp(sm, wts, tid, ScratchRecord{scr});
@@ -927,7 +938,7 @@ render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const
                 *reinterpret_cast<float2*>(s_df + (64 * wg + 16 * w + g + 8 * hh) * 8 + 2 * q) =
                     make_float2(d1[0][2 * hh] * sc_m, d1[0][2 * hh + 1] * sc_m);
             __syncthreads();
-            if (tid < TILE_M && valid) volume_scatter<DET>(sc, io, bw, s_df, si, tid, det);
+            if (tid < TILE_M && valid) volume_scatter<DET, FAST>(sc, io, bw, s_df, si, tid, det, scr);
         }
         __syncthreads();
     }
@@ -1008,11 +1019,20 @@ __device__ __forceinline__ int det_scale_exp(unsigned amax_bits, long long n) {
     return 61 - k - em;                                         // -106 <= e <= 188 for n <= 2^40: a double scale
 }
 
+// FAST (the rays entry): each sample's NDC is marched again from io.rays / io.t_steps / jitter by the function the
+// backward kernel's front end used (sample_point), so it has the same bits and needs no per-sample record.
+template <bool FAST>
 __global__ void det_scatter_kernel(const SceneDev sc, const float* __restrict__ ndc, const float* __restrict__ rec,
                                    const unsigned* __restrict__ amax, long long nsamp,
-                                   unsigned long long* __restrict__ acc, float* __restrict__ dvol) {
+                                   unsigned long long* __restrict__ acc, float* __restrict__ dvol, const RenderIO io,
+                                   const float* __restrict__ jitter) {
     const unsigned mb = amax[0];
     if (mb == 0u && amax[1] == 0u) return;                      // all-zero gradients
+    __shared__ Cams cams;
+    if constexpr (FAST) {
+        load_cams(sc, &cams, threadIdx.x);
+        __syncthreads();
+    }
     const double s = __longlong_as_double((long long)(1023 + det_scale_exp(mb, nsamp)) << 52);
     const int W = sc.Wp, H = sc.Hp, D = sc.D;
     // thread t: sample t >> 6, corner (t >> 3) & 7, channel t & 7 -- a warp adds 4 corners x 64 contiguous bytes
@@ -1021,7 +1041,15 @@ __global__ void det_scatter_kernel(const SceneDev sc, const float* __restrict__ 
         const int c = (int)(t >> 3) & 7, ch = (int)t & 7;
         const float g = __ldg(rec + si * 8 + ch);
         if (g == 0.f) continue;
-        const Trilinear tr = trilinear_corners(sc, __ldg(ndc + si * 3), __ldg(ndc + si * 3 + 1), __ldg(ndc + si * 3 + 2));
+        Trilinear tr;
+        if constexpr (FAST) {
+            const int ray = (int)(si / io.S), s_idx = (int)(si - (long long)ray * io.S);
+            float px, py, pz, dx, dy, dz, nx, ny, nz, z;
+            sample_point<true, true>(sc, cams, io, ray, s_idx, (size_t)si, px, py, pz, dx, dy, dz, nx, ny, nz, z, jitter);
+            tr = trilinear_corners(sc, nx, ny, nz);
+        } else {
+            tr = trilinear_corners(sc, __ldg(ndc + si * 3), __ldg(ndc + si * 3 + 1), __ldg(ndc + si * 3 + 2));
+        }
         const int x = tr.x0 + (c & 1), y = tr.y0 + ((c >> 1) & 1), z = tr.z0 + (c >> 2);
         if ((unsigned)x >= (unsigned)W || (unsigned)y >= (unsigned)H || (unsigned)z >= (unsigned)D) continue;   // zeros padding
         const float wgt = tr.wx[c & 1] * tr.wy[(c >> 1) & 1] * tr.wz[c >> 2];
@@ -1067,6 +1095,24 @@ static int bwd_grid(int N, int S) {
     return ngroups < sm_count() ? ngroups : sm_count();
 }
 
+// One backward-kernel launch of the variant (tc, DET, FAST); wh is the fp16 dgrad image (tc) or unused.
+template <bool DET, bool FAST>
+static int launch_bwd_kernel(bool tc, int grid, const SceneDev& sc, const RenderIO& io, const BwdIO& bw, const float* wts,
+                             const __half* wh, const DetIO& dt, const float* jitter, cudaStream_t stream) {
+    static bool attr_set[2][64] = {};
+    const void* kfn = tc ? (const void*)render_bwd_tc_kernel<DET, FAST> : (const void*)render_bwd_kernel<DET, FAST>;
+    int dev = 0;
+    MVSN_CUDA_CHECK(cudaGetDevice(&dev));
+    if (dev >= 64 || !attr_set[tc][dev]) {
+        MVSN_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+        if (dev < 64) attr_set[tc][dev] = true;
+    }
+    if (tc) render_bwd_tc_kernel<DET, FAST><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts, wh, dt, jitter);
+    else    render_bwd_kernel<DET, FAST><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts, dt, jitter);
+    MVSN_CUDA_CHECK(cudaGetLastError());
+    return MVSN_OK;
+}
+
 }  // namespace
 
 size_t render_backward_workspace_bytes(int N, int S) {
@@ -1110,9 +1156,11 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
                            const float* g_rgb, const float* target, float inv_count, const float* g_depth,
                            const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
                            float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det) {
-    const char* what = det ? (tc ? "deterministic render backward (grad_mode TC_HALF)" : "deterministic render backward")
-                           : (tc ? "render backward (grad_mode TC_HALF)" : "render backward");
+                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det, const float* jitter) {
+    const bool fast = io.rays != nullptr;
+    const char* what = fast ? "mvsn_render_backward_rays"
+                            : det ? (tc ? "deterministic render backward (grad_mode TC_HALF)" : "deterministic render backward")
+                                  : (tc ? "render backward (grad_mode TC_HALF)" : "render backward");
     MVSN_REQUIRE(io.S <= TILE_M, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, io.S);
     const size_t base = tc ? render_backward_tc_workspace_bytes(io.N, io.S) : render_backward_workspace_bytes(io.N, io.S);
     const size_t nvox = dvol ? (size_t)sc.D * sc.Hp * sc.Wp : 0;
@@ -1120,16 +1168,6 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
     const size_t need = det ? dl.total : base;
     MVSN_REQUIRE(workspace && workspace_bytes >= need, MVSN_EWORKSPACE, "%s: workspace %zu < %zu bytes", what, workspace_bytes, need);
     MVSN_REQUIRE(aligned16(workspace), MVSN_EALIGN, "%s: workspace must be 16-byte aligned", what);
-    static bool attr_set[4][64] = {};
-    const int kind = (tc ? 2 : 0) + (det ? 1 : 0);
-    int dev = 0;
-    MVSN_CUDA_CHECK(cudaGetDevice(&dev));
-    if (dev >= 64 || !attr_set[kind][dev]) {
-        const void* kfn = tc ? (det ? (const void*)render_bwd_tc_kernel<true> : (const void*)render_bwd_tc_kernel<false>)
-                             : (det ? (const void*)render_bwd_kernel<true> : (const void*)render_bwd_kernel<false>);
-        MVSN_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
-        if (dev < 64) attr_set[kind][dev] = true;
-    }
     DetIO dt{};
     if (det) {
         char* w8 = static_cast<char*>(workspace);
@@ -1151,20 +1189,19 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
     float* wimg = ws + ctas * (bwd::SCRATCH + bwd::GRADS);   // the dgrad weight image: fp32, or fp16 for the tc kernel
     MlpPtrsB wp;
     for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) wp.p[i] = mlp_w[i];
+    __half* wh = reinterpret_cast<__half*>(wimg);
     if (tc) {
-        __half* wh = reinterpret_cast<__half*>(wimg);
         pack_dgrad_half_kernel<<<64, 256, 0, stream>>>(wp, wh);
-        MVSN_CUDA_CHECK(cudaGetLastError());
-        if (det) render_bwd_tc_kernel<true><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, wh, dt);
-        else     render_bwd_tc_kernel<false><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, wh, dt);
     } else {
         bw.wd = wimg;
         pack_dgrad_kernel<<<64, 256, 0, stream>>>(wp, wimg);
-        MVSN_CUDA_CHECK(cudaGetLastError());
-        if (det) render_bwd_kernel<true><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, dt);
-        else     render_bwd_kernel<false><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts_fp32, dt);
     }
     MVSN_CUDA_CHECK(cudaGetLastError());
+    const int rc = det ? (fast ? launch_bwd_kernel<true, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
+                               : launch_bwd_kernel<true, false>(tc, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream))
+                       : (fast ? launch_bwd_kernel<false, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
+                               : launch_bwd_kernel<false, false>(tc, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream));
+    if (rc) return rc;
     GradOut go;
     for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) go.p[i] = grad_mlp[i];
     mlp_grad_reduce_kernel<<<dim3(16, MVSN_N_MLP_TENSORS), 256, 0, stream>>>(bw.grads, grid, go);
@@ -1173,7 +1210,8 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
         const long long nsamp = (long long)io.N * io.S;
         auto* acc = reinterpret_cast<unsigned long long*>(static_cast<char*>(workspace) + dl.acc);
         const int gs = cdiv(nsamp * 64, 256) < sm_count() * 16 ? cdiv(nsamp * 64, 256) : sm_count() * 16;
-        det_scatter_kernel<<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, dvol);
+        if (fast) det_scatter_kernel<true><<<gs, 256, 0, stream>>>(sc, nullptr, dt.rec, dt.amax, nsamp, acc, dvol, io, jitter);
+        else      det_scatter_kernel<false><<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, dvol, io, nullptr);
         MVSN_CUDA_CHECK(cudaGetLastError());
         const long long n2 = (long long)nvox * 4;               // (int64 pair, float pair) per thread step
         const int gc = cdiv(n2, 256) < sm_count() * 8 ? cdiv(n2, 256) : sm_count() * 8;

@@ -69,7 +69,9 @@ int launch_render_wg(const SceneDev& sc, const RenderIO& io, bool fast, bool spl
 size_t mlp_wg_packed_bytes(bool split);
 int pack_mlp_wg(const float* const* w, bool split, void* packed, cudaStream_t stream);
 // fine-tuning step (render_bwd.cu); tc: dgrad / wgrad GEMMs on wgmma with fp16 operands (grad_mode TC_HALF);
-// det: the volume gradient and the loss summed in a fixed order (bit-reproducible)
+// det: the volume gradient and the loss summed in a fixed order (bit-reproducible); io.rays set: the samples are
+// marched in the kernel from io.rays / io.t_steps, stratified by `jitter` [N,S] (NULL: none), instead of read from
+// io.pts / io.ndc / io.z / io.dirs
 size_t render_backward_workspace_bytes(int N, int S);
 size_t render_backward_tc_workspace_bytes(int N, int S);
 size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc);
@@ -77,7 +79,8 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
                            const float* g_rgb, const float* target, float inv_count, const float* g_depth,
                            const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
                            float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det);
+                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det,
+                           const float* jitter = nullptr);
 int launch_adam_tensors(float* const* p, const float* const* g, float* const* m, float* const* v, const int* n, int count,
                         float lr, float beta1, float beta2, float eps, int step, cudaStream_t stream);
 int launch_adam_volume(float* p, float* g_dhwc, float* m, float* v, long long nvox, int planar, float lr, float beta1,
@@ -133,17 +136,30 @@ __device__ __forceinline__ float ray_z(float near, float far, float t, int lindi
     return __fdiv_rn(1.f, __fadd_rn(__fmul_rn(__fdiv_rn(1.f, near), 1.f - t), __fmul_rn(__fdiv_rn(1.f, far), t)));
 }
 
+// stratified depth of sample s of S (data/ray_utils.py:184-191, perturb > 0): lower + (upper - lower) j, between the
+// midpoints of the neighbouring ray_z depths (lower = z_0 for s = 0, upper = z_{S-1} for s = S - 1), j = perturb * u.
+// Every operation rounded on its own, as ray_marcher's element-wise PyTorch ops round them.
+__device__ __forceinline__ float ray_z_jittered(float near, float far, const float* t_steps, int s, int S, int lindisp,
+                                                float j) {
+    const float z = ray_z(near, far, __ldg(t_steps + s), lindisp);
+    const float lower = s == 0 ? z : __fmul_rn(0.5f, __fadd_rn(ray_z(near, far, __ldg(t_steps + s - 1), lindisp), z));
+    const float upper = s == S - 1 ? z : __fmul_rn(0.5f, __fadd_rn(z, ray_z(near, far, __ldg(t_steps + s + 1), lindisp)));
+    return __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), j));
+}
+
 // ray-march point (px, py, pz), ray direction (dx, dy, dz), NDC (nx, ny, nz) and depth z of sample s_idx of ray `ray`:
-// marched from io.rays / io.t_steps (FAST) or read from the caller's per-sample arrays (si = ray * S + s_idx)
+// marched from io.rays / io.t_steps (FAST) or read from the caller's per-sample arrays (si = ray * S + s_idx).
+// FAST with `jitter` ([N,S], the fine-tuning backward): the stratified depth ray_z_jittered with j = jitter[si].
 template <bool FAST, bool PRECISE>
 __device__ __forceinline__ void sample_point(const SceneDev& sc, const Cams& cams, const RenderIO& io, int ray, int s_idx,
                                              size_t si, float& px, float& py, float& pz, float& dx, float& dy, float& dz,
-                                             float& nx, float& ny, float& nz, float& z) {
+                                             float& nx, float& ny, float& nz, float& z, const float* jitter = nullptr) {
     if (FAST) {
         const float4* rp = reinterpret_cast<const float4*>(io.rays + (size_t)ray * 8);
         float4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
         dx = r0.w; dy = r1.x; dz = r1.y;
-        z = ray_z(r1.z, r1.w, __ldg(io.t_steps + s_idx), io.rg.lindisp);
+        if (jitter) z = ray_z_jittered(r1.z, r1.w, io.t_steps, s_idx, io.S, io.rg.lindisp, __ldg(jitter + si));
+        else        z = ray_z(r1.z, r1.w, __ldg(io.t_steps + s_idx), io.rg.lindisp);
         px = __fadd_rn(r0.x, __fmul_rn(dx, z));
         py = __fadd_rn(r0.y, __fmul_rn(dy, z));
         pz = __fadd_rn(r0.z, __fmul_rn(dz, z));

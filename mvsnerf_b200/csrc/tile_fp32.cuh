@@ -150,16 +150,18 @@ __device__ __forceinline__ void epilogue128(float (&acc)[8][8], const float* __r
 // Front end of row `row` (threads 0..127): sample s_idx of ray `ray`, as the caller maps rows to samples.  Fills the
 // row of sm.pe, the FEAT_LD feature row at the start of sm.h, sm.dir and sm.z; an invalid row gets zeros (and
 // cos(0) = 1 in its positional encoding).  With io.input_feat set, the 20 feature channels also go to HBM.
+// `jitter`: stratified depths for the FAST march (see sample_point).
 template <bool FAST, class Rec>
 __device__ __forceinline__ void tile_front_end(const SceneDev& sc, const Cams& cams, const RenderIO& io, const TileSmem& sm,
-                                               int row, int ray, int s_idx, bool valid, const Rec& rec) {
+                                               int row, int ray, int s_idx, bool valid, const Rec& rec,
+                                               const float* jitter = nullptr) {
     float pe[3] = {0.f, 0.f, 0.f}, feat[20], dir[3] = {0.f, 0.f, 0.f}, zv = 0.f;
 #pragma unroll
     for (int i = 0; i < 20; ++i) feat[i] = 0.f;
     if (valid) {
         const size_t si = (size_t)ray * io.S + s_idx;
         float px, py, pz, dx, dy, dz;
-        sample_point<FAST, true>(sc, cams, io, ray, s_idx, si, px, py, pz, dx, dy, dz, pe[0], pe[1], pe[2], zv);
+        sample_point<FAST, true>(sc, cams, io, ray, s_idx, si, px, py, pz, dx, dy, dz, pe[0], pe[1], pe[2], zv, jitter);
         view_dir(cams, dx, dy, dz, dir);
         sample_volume(sc, pe[0], pe[1], pe[2], feat);
 #pragma unroll

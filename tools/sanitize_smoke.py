@@ -55,5 +55,12 @@ if not only or "backward" in only:
                                              torch.tensor([sc.W - 1.0, sc.H - 1.0], device=dev), near=sc.near_far[0],
                                              far=sc.near_far[1], pad=sc.pad)
             tuner.step(xyz, ndc, z, rd, torch.rand(37, 3, device=dev), want_forward=True)
+            # the same step from rays (mvsn_render_backward_rays), with and without jitter, then deterministic
+            tuner.step_rays(rays[:37], torch.rand(37, 3, device=dev), sc.near_far, float(sc.pad), N_samples=S,
+                            want_forward=True)
+            tuner.step_rays(rays[:37], torch.rand(37, 3, device=dev), sc.near_far, float(sc.pad), N_samples=S, perturb=0.0)
+            torch.use_deterministic_algorithms(True, warn_only=True)
+            tuner.step_rays(rays[:37], torch.rand(37, 3, device=dev), sc.near_far, float(sc.pad), N_samples=S)
+            torch.use_deterministic_algorithms(False)
 torch.cuda.synchronize()
 print("sanitize_smoke: done")
