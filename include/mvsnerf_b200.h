@@ -127,6 +127,20 @@ int mvsn_render_rays(const mvsn_render_scene* scene, const mvsn_ray_params* rp,
                      float* rgb, float* depth, float* weights, float* alpha, float* input_feat,
                      void* stream);
 
+/* mvsn_render_rays_stop: mvsn_render_rays (rgb and depth only) with early ray termination.  Rays are composited in
+ * groups of up to 32 neighbours, two samples per tile at frame sizes; after compositing tile k of a group, if every ray
+ * of the group has transmittance T < t_stop, the group's tiles k + 3 onwards are not computed and each pixel is the
+ * prefix of mvsn_render_rays' sums (same order, same arithmetic).  The omitted tail weighs less than t_stop: per
+ * channel, -t_stop < rgb - rgb_full <= 0 (white_bkgd: 0 <= rgb - rgb_full < t_stop), 0 <= depth_full - depth <
+ * t_stop * far.  t_stop = 0 never stops (bit-identical to mvsn_render_rays).  A group's result depends on its own rays
+ * only, so frames are bit-reproducible.  tiles_done (device, 8-byte aligned, may be NULL): += the number of 64-sample
+ * tiles computed.
+ * Modes MVSN_MLP_TC_HALF / TC_PAIR / TC_SPLIT; MVSN_MLP_FP32 gives MVSN_EUNSUPPORTED.  Argument errors (NULL pointers,
+ * t_stop negative or NaN, the mode, a misaligned rays or tiles_done) are returned before any CUDA call. */
+int mvsn_render_rays_stop(const mvsn_render_scene* scene, const mvsn_ray_params* rp,
+                          const float* rays, const float* t_steps, int N, int S, float t_stop,
+                          float* rgb, float* depth, unsigned long long* tiles_done, void* stream);
+
 /* Ray generation for one camera (replaces: data/ray_utils.get_rays, data/ray_utils.py:32-53, and the notebooks'
  * `torch.cat([rays_o, rays_d, near, far])`): directions [n,3] = get_ray_directions(H, W, focal) in camera coordinates
  * (resident on the device, they depend on the intrinsics only), c2w = the first three rows of the camera-to-world matrix,

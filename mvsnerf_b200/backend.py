@@ -988,7 +988,7 @@ _tsteps = {}
 
 
 def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad, N_samples=128,
-                white_bkgd=False, lindisp=False, mlp_mode=None, out=None, sink=None):
+                white_bkgd=False, lindisp=False, mlp_mode=None, out=None, sink=None, t_stop=None, tiles_done=None):
     """Fused-caller entry: one launch renders all `rays` [N,8] = (o, d, near, far).
 
     Replaces the notebooks' per-chunk loop `ray_marcher -> get_ndc_coordinate -> rendering`
@@ -998,9 +998,25 @@ def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
 
     `sink` (a lib.PeerSink from distributed.PeerFrame.sink): the kernel epilogue additionally stores every pixel
     as (r, g, b, depth) into all ranks' copies of the assembled frame (mvsn_render_rays_to_peers); with a sink and
-    no `out`, nothing else is written and (None, None) is returned."""
+    no `out`, nothing else is written and (None, None) is returned.
+
+    `t_stop` (a float >= 0, tensor-core modes): early ray termination (mvsn_render_rays_stop) -- a group of up to 32
+    neighbouring rays stops two tiles (four samples at frame sizes) after every ray in it has transmittance < t_stop, so
+    each channel differs from the full render by less than t_stop (t_stop = 0: bit-identical).  `tiles_done`: an
+    optional CUDA int64 tensor [1] the number of computed 64-sample tiles is added to.  Not combinable with `sink`."""
     lib = _lib.load()
     mode = DEFAULT_MLP_MODE if mlp_mode is None else mlp_mode
+    if t_stop is not None:
+        t_stop = float(t_stop)
+        if sink is not None:
+            raise RuntimeError("render_rays: t_stop cannot be combined with sink (peer frame assembly)")
+        if mode == _lib.MLP_FP32:
+            raise RuntimeError("render_rays: t_stop needs a tensor-core mlp_mode (MLP_TC_HALF / TC_PAIR / TC_SPLIT)")
+        if tiles_done is not None and (not tiles_done.is_cuda or tiles_done.device != rays.device
+                                       or tiles_done.dtype != torch.int64 or tiles_done.numel() < 1):
+            raise RuntimeError(f"render_rays: tiles_done must be a CUDA int64 tensor on the rays' device ({rays.device})")
+    elif tiles_done is not None:
+        raise RuntimeError("render_rays: tiles_done needs t_stop")
     rays = _lib.dev_f32(rays, "rays")
     N = rays.shape[0]
     dev = rays.device
@@ -1016,7 +1032,12 @@ def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
         rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
         depth = torch.empty(N, dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        if sink is not None:
+        if t_stop is not None:
+            _lib.check(lib.mvsn_render_rays_stop(C.byref(sc), C.byref(rp), _lib.ptr(rays), _lib.ptr(t_steps), N, S,
+                                                 t_stop, _lib.ptr(rgb), _lib.ptr(depth), _lib.ptr(tiles_done),
+                                                 _lib.stream_ptr()),
+                       "mvsn_render_rays_stop")
+        elif sink is not None:
             _lib.check(lib.mvsn_render_rays_to_peers(C.byref(sc), C.byref(rp), _lib.ptr(rays), _lib.ptr(t_steps), N, S,
                                                      C.byref(sink), _lib.ptr(rgb), _lib.ptr(depth), _lib.stream_ptr()),
                        "mvsn_render_rays_to_peers")

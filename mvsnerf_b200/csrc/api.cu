@@ -293,6 +293,34 @@ int mvsn_render_rays(const mvsn_render_scene* scene, const mvsn_ray_params* rp, 
     return render_rays_impl(scene, rp, rays, t_steps, N, S, rgb, depth, weights, alpha, input_feat, nullptr, stream);
 }
 
+int mvsn_render_rays_stop(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const float* rays,
+                          const float* t_steps, int N, int S, float t_stop, float* rgb, float* depth,
+                          unsigned long long* tiles_done, void* stream) {
+    MVSN_RANGE("mvsn_render_rays_stop");
+    SceneDev sc;
+    int rc = make_scene(scene, sc);
+    if (rc) return rc;
+    MVSN_REQUIRE(rp != nullptr, MVSN_ENULL, "mvsn_render_rays_stop: ray params NULL");
+    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "mvsn_render_rays_stop: N=%d S=%d", N, S);
+    MVSN_REQUIRE(rays && t_steps && rgb && depth, MVSN_ENULL, "mvsn_render_rays_stop: NULL required pointer");
+    MVSN_REQUIRE(t_stop >= 0.f, MVSN_EBADSHAPE, "mvsn_render_rays_stop: t_stop=%g must be >= 0 (not NaN)", (double)t_stop);
+    MVSN_REQUIRE(scene->mlp_mode == MVSN_MLP_TC_HALF || scene->mlp_mode == MVSN_MLP_TC_PAIR ||
+                     scene->mlp_mode == MVSN_MLP_TC_SPLIT,
+                 MVSN_EUNSUPPORTED, "mvsn_render_rays_stop: mlp_mode %d has no early ray termination (tensor-core modes only)",
+                 scene->mlp_mode);
+    MVSN_REQUIRE(aligned16(rays), MVSN_EALIGN, "rays must be 16-byte aligned");
+    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(tiles_done) % 8 == 0, MVSN_EALIGN,
+                 "mvsn_render_rays_stop: tiles_done must be 8-byte aligned");
+    if (N == 0) return MVSN_OK;
+    RenderIO io{};
+    io.rays = rays; io.t_steps = t_steps;
+    io.N = N; io.S = S;
+    io.rgb = rgb; io.depth = depth;
+    io.rg = make_ray_gen(scene, rp);
+    return launch_render_wg(sc, io, true, scene->mlp_mode == MVSN_MLP_TC_SPLIT, scene->mlp_packed, (cudaStream_t)stream,
+                            &t_stop, tiles_done);
+}
+
 int mvsn_render_rays_to_peers(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const float* rays,
                               const float* t_steps, int N, int S, const mvsn_peer_sink* sink, float* rgb,
                               float* depth, void* stream) {

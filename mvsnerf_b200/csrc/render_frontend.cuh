@@ -64,8 +64,10 @@ __device__ __forceinline__ void store_pixel(const RenderIO& io, int ray, float r
 }
 
 int launch_render_fp32(const SceneDev& sc, const RenderIO& io, bool fast, const float* wts, cudaStream_t stream);
-// tensor-core modes (render_wg.cu): split = MVSN_MLP_TC_SPLIT, otherwise the fp16-operand modes
-int launch_render_wg(const SceneDev& sc, const RenderIO& io, bool fast, bool split, const void* wimg, cudaStream_t stream);
+// tensor-core modes (render_wg.cu): split = MVSN_MLP_TC_SPLIT, otherwise the fp16-operand modes.  t_stop != NULL
+// (fast only): early ray termination at transmittance *t_stop; tiles_done (may be NULL) += the tiles computed
+int launch_render_wg(const SceneDev& sc, const RenderIO& io, bool fast, bool split, const void* wimg, cudaStream_t stream,
+                     const float* t_stop = nullptr, unsigned long long* tiles_done = nullptr);
 size_t mlp_wg_packed_bytes(bool split);
 int pack_mlp_wg(const float* const* w, bool split, void* packed, cudaStream_t stream);
 // fine-tuning step (render_bwd.cu); tc: dgrad / wgrad GEMMs on wgmma with fp16 operands (grad_mode TC_HALF);

@@ -78,6 +78,11 @@ __host__ __device__ constexpr int smem_bytes(bool split) { return off_bias(split
 static_assert(smem_bytes(false) <= 227 * 1024 && smem_bytes(true) <= 227 * 1024, "shared memory budget");
 static_assert(wg_bytes(true) % 1024 == 0 && SLOT_BYTES % 1024 == 0 && off_ring(false) % 1024 == 0,
               "SW128 tiles need 1024-byte alignment");
+// early ray termination (STOP launches only): the pass protocol's state after the biases
+constexpr int STOP_BYTES = 128;
+__host__ __device__ constexpr int off_stop(bool split) { return off_bias(split) + BIAS_FLOATS * 4; }
+static_assert(smem_bytes(false) + STOP_BYTES <= 227 * 1024 && smem_bytes(true) + STOP_BYTES <= 227 * 1024,
+              "shared memory budget");
 }  // namespace wg
 
 struct WgShared {
@@ -87,6 +92,29 @@ struct WgShared {
     uint64_t slot_empty[wg::SLOTS];
     Cams cams;
 };
+
+// STOP: every consumer publishes, at the start of pass p, what it computes in pass p + 2 (its plan); dec[(p + 2) & 3]
+// completes when all consumers have (the plans of passes 0 and 1 are set up before the roles split).  The loader, the
+// producer and idle consumers read the plans of a pass only after that barrier.  Four slots: a slot is rewritten two
+// passes after the pass it plans, when every reader of it is provably done (see DESIGN §4 K-C).
+constexpr int STOP_SLOTS = 4;
+struct WgStop {
+    uint64_t dec[STOP_SLOTS];
+    int2 plan[STOP_SLOTS][wg::NWG];                        // (group, tile) of consumer w in pass p (slot p & 3); group -1: idle
+    int next;                                              // next index into the CTA's group list
+};
+static_assert(sizeof(WgStop) <= wg::STOP_BYTES, "stop state");
+__device__ __forceinline__ WgStop* stop_state(uint8_t* smem, bool split) { return reinterpret_cast<WgStop*>(smem + wg::off_stop(split)); }
+// index j of the CTA's group list -> group: the groups the static decomposition gives this CTA, in order
+__device__ __forceinline__ int stop_group(int j) {
+    return ((j / wg::NWG) * (int)gridDim.x + (int)blockIdx.x) * wg::NWG + j % wg::NWG;
+}
+// wait for the plans of pass p >= 2 (published at the start of pass p - 2: completion (p - 2) / 4 of dec[p & 3])
+__device__ __forceinline__ void stop_wait(WgStop* ss, int pass) {
+    if (pass >= 2) mbar_wait(&ss->dec[pass & (STOP_SLOTS - 1)], ((pass - 2) >> 2) & 1);
+}
+__device__ __forceinline__ int2 stop_plan(const WgStop* ss, int pass, int w) { return ss->plan[pass & (STOP_SLOTS - 1)][w]; }
+__device__ __forceinline__ bool stop_busy(const WgStop* ss, int pass, int w) { return stop_plan(ss, pass, w).x >= 0; }
 
 __device__ __forceinline__ uint32_t pack_h2_rn(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
@@ -308,9 +336,22 @@ __device__ __forceinline__ void front_end(const SceneDev& sc, const Cams& cams, 
     }
 }
 
-template <bool FAST, bool SPLIT>
+// STOP: the state a consumer carries from pass to pass -- the verdict of the tile composited last (warp 0: every valid
+// ray of the group has cT < t_stop), no work left, the current tile is its group's last, tiles computed
+template <bool STOP> struct StopRegs { bool verdict = false, idle = false, last = false; uint32_t ncomp = 0; };
+template <> struct StopRegs<false> { static constexpr bool last = false; };
+
+// STOP (early ray termination, FAST only): after compositing tile k of a group, if every valid ray of the group has
+// transmittance cT < t_stop, the group's tiles k + 3 onwards are not computed (k + 1 and k + 2 are composited as
+// usual), and the number of passes of a CTA becomes dynamic.  Each consumer computes its plan for pass p + 2 at the
+// start of pass p: the next tile of its group, or the next group of the CTA's list (a shared counter, in order of
+// demand), or idle.  Tile k + 2 depends only on the verdicts up to tile k - 1, so every plan is known two passes ahead
+// and the producer fills a slot as soon as its consumer releases it, as without STOP.  Without STOP the kernel is the
+// one it always was (t_stop and tiles_done are unused).
+template <bool FAST, bool SPLIT, bool STOP = false>
 __global__ void __launch_bounds__(wg::threads(SPLIT), 1)
-render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict__ wimg) {
+render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict__ wimg, float t_stop,
+                 unsigned long long* tiles_done) {
     using namespace wg;
     constexpr int NS = nstage(SPLIT), THREADS = threads(SPLIT);
     extern __shared__ uint8_t smem_raw[];
@@ -325,6 +366,21 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         for (int i = 0; i < NS; ++i) { mbar_init(&sh.full[i], 1); mbar_init(&sh.empty[i], NWG * 4); }
         if (!SPLIT)
             for (int i = 0; i < SLOTS; ++i) { mbar_init(&sh.slot_full[i], 128); mbar_init(&sh.slot_empty[i], 4); }
+        if constexpr (STOP) {
+            WgStop* ss = stop_state(smem, SPLIT);
+            const int G0 = (io.N + io.rays_per_tile - 1) / io.rays_per_tile;
+            const int NT0 = (io.S + wg::ROWS / io.rays_per_tile - 1) / (wg::ROWS / io.rays_per_tile);
+            for (int i = 0; i < STOP_SLOTS; ++i) mbar_init(&ss->dec[i], NWG);
+            int next = NWG;                              // passes 0 and 1: first groups, then their tile 1 (or the next group)
+            for (int w = 0; w < NWG; ++w) {
+                const int g0 = stop_group(w) < G0 ? stop_group(w) : -1;
+                ss->plan[0][w] = make_int2(g0, 0);
+                int2 p1 = make_int2(g0, 1);
+                if (g0 >= 0 && NT0 == 1) { const int gn = stop_group(next++); p1 = make_int2(gn < G0 ? gn : -1, 0); }
+                ss->plan[1][w] = g0 < 0 ? make_int2(-1, 0) : p1;
+            }
+            ss->next = next;
+        }
         fence_barrier_init();
     }
     __syncthreads();
@@ -347,7 +403,15 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         if (elect_one()) {
             uint32_t n = 0;
 #pragma unroll 1
-            for (int pass = 0; pass < npass; ++pass) {
+            for (int pass = 0; STOP || pass < npass; ++pass) {
+                if constexpr (STOP) {                    // one pass of NCHUNK chunks while any consumer has work
+                    WgStop* ss = stop_state(smem, SPLIT);
+                    stop_wait(ss, pass);
+                    bool any = false;
+#pragma unroll
+                    for (int w = 0; w < NWG; ++w) any |= stop_busy(ss, pass, w);
+                    if (!any) break;
+                }
 #pragma unroll 1
                 for (int c = 0; c < NCHUNK; ++c, ++n) {
                     const uint32_t st = n % NS;
@@ -372,15 +436,24 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
 #pragma unroll
             for (int w = 0; w < NWG; ++w) filled[w] = 0;
 #pragma unroll 1
-            for (int pass = 0; pass < npass; ++pass) {
+            for (int pass = 0; STOP || pass < npass; ++pass) {
+                int2 pl[NWG];                            // STOP: the consumers' plans for this pass
+                if constexpr (STOP) {
+                    WgStop* ss = stop_state(smem, SPLIT);
+                    stop_wait(ss, pass);
+                    bool any = false;
+#pragma unroll
+                    for (int w = 0; w < NWG; ++w) { pl[w] = stop_plan(ss, pass, w); any |= pl[w].x >= 0; }
+                    if (!any) break;
+                }
 #pragma unroll
                 for (int w = 0; w < NWG; ++w) {
-                    const int grp = group_of(pass, w);
-                    if (grp >= G) continue;
+                    const int grp = STOP ? pl[w].x : group_of(pass, w);
+                    if (STOP ? grp < 0 : grp >= G) continue;
                     const int s = 2 * w + (filled[w] & 1);
                     if (filled[w] >= 2) mbar_wait(&sh.slot_empty[s], ((filled[w] >> 1) - 1) & 1);
                     uint8_t* pe = smem + s * SLOT_BYTES;
-                    front_end<FAST, false>(sc, sh.cams, io, grp, pass % NT, t, pe, pe + tile_bytes(false));
+                    front_end<FAST, false>(sc, sh.cams, io, grp, STOP ? pl[w].y : pass % NT, t, pe, pe + tile_bytes(false));
                     fence_proxy_async();
                     mbar_arrive(&sh.slot_full[s]);
                     ++filled[w];
@@ -417,13 +490,53 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
     const float inv_w = SPLIT ? bias[BIAS_WINV] : 1.f;
     float sa = 1.f, sb = 1.f, ia = inv_w, ib = inv_w;
 
+    StopRegs<STOP> sr;
+
 #pragma unroll 1
-    for (int pass = 0; pass < npass; ++pass) {
-        const int grp = group_of(pass, wgi), tile = pass % NT;
-        if (grp >= G) {                                  // idle in the final passes: keep the weight ring moving
+    for (int pass = 0; STOP || pass < npass; ++pass) {
+        int grp = group_of(pass, wgi), tile = pass % NT;
+        if constexpr (STOP) {
+            WgStop* ss = stop_state(smem, SPLIT);
+            if (!sr.idle) {                              // own plans: written by thread 0 before named barriers
+                const int2 pl = stop_plan(ss, pass, wgi);
+                grp = pl.x; tile = pl.y; sr.idle = grp < 0;
+            }
+            if (sr.idle) {                                  // keep the weight ring moving while another consumer works
+                stop_wait(ss, pass);
+                bool any = false;
+#pragma unroll
+                for (int w = 0; w < NWG; ++w) any |= w != wgi && stop_busy(ss, pass, w);
+                if (!any) break;
+                if (t == 0) {
+                    ss->plan[(pass + 2) & (STOP_SLOTS - 1)][wgi] = make_int2(-1, 0);
+                    mbar_arrive(&ss->dec[(pass + 2) & (STOP_SLOTS - 1)]);
+                }
 #pragma unroll 1
-            for (int c = 0; c < NCHUNK; ++c) { acquire(); release(); }
-            continue;
+                for (int c = 0; c < NCHUNK; ++c) { acquire(); release(); }
+                continue;
+            }
+            // from the plan of pass + 1, (g, k): tile k + 1 of g is skipped iff k + 1 == NT or the verdict of tile k - 2
+            // (this consumer's last composited tile) says stop
+            if (t == 0) {
+                const int2 p1 = stop_plan(ss, pass + 1, wgi);
+                int2 nx = make_int2(-1, 0);
+                if (p1.x >= 0) {
+                    nx = make_int2(p1.x, p1.y + 1);
+                    if (p1.y + 1 >= NT || (p1.y >= 2 && sr.verdict)) {
+                        const int gn = stop_group(atomicAdd(&ss->next, 1));
+                        nx = make_int2(gn < G ? gn : -1, 0);
+                    }
+                }
+                ss->plan[(pass + 2) & (STOP_SLOTS - 1)][wgi] = nx;
+                mbar_arrive(&ss->dec[(pass + 2) & (STOP_SLOTS - 1)]);
+            }
+            ++sr.ncomp;
+        } else {
+            if (grp >= G) {                              // idle in the final passes: keep the weight ring moving
+#pragma unroll 1
+                for (int c = 0; c < NCHUNK; ++c) { acquire(); release(); }
+                continue;
+            }
         }
         uint32_t pe_u, misc_u, slot = 0;
         named_bar_sync(1 + wgi, 128);                    // the previous tile's exchange (split: operand tiles) is consumed
@@ -577,6 +690,10 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             }
         }
         named_bar_sync(1 + wgi, 128);
+        if constexpr (STOP) {                            // the group's last tile unless pass + 1 plans (grp, tile + 1)
+            const int2 p1 = stop_plan(stop_state(smem, SPLIT), pass + 1, wgi);
+            sr.last = !(p1.x == grp && p1.y == tile + 1);
+        }
         // -------------------------- compositing (renderer.py:18-26,65-92) ----------------------------------
         // the first RT threads walk their ray's SP samples of this tile front to back -- the reference's
         // sequential cumprod order
@@ -600,17 +717,24 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                     c3 = fmaf(wgt, z, c3); c4 += wgt;
                     cT *= (1.f - v.x) + 1e-10f;
                 }
-                if (tile == NT - 1) {
+                if (STOP ? sr.last : tile == NT - 1) {
                     float o0 = c0, o1 = c1, o2 = c2;
                     if (sc.white_bkgd) { const float bg = 1.f - c4; o0 += bg; o1 += bg; o2 += bg; }
                     store_pixel(io, cray, o0, o1, o2, c3);
                 }
             }
         }
+        if constexpr (STOP) {                            // rays past the batch end (and lanes >= RT) count as stopped
+            if (t < 32) sr.verdict = __all_sync(0xffffffffu, t >= RT || grp * RT + t >= N || cT < t_stop);
+        }
+    }
+    if constexpr (STOP) {
+        if (t == 0 && tiles_done) atomicAdd(tiles_done, (unsigned long long)sr.ncomp);
     }
 }
 
-int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool split, const void* wimg, cudaStream_t stream) {
+int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool split, const void* wimg, cudaStream_t stream,
+                     const float* t_stop, unsigned long long* tiles_done) {
     using namespace wg;
     RenderIO io = io_in;
     static bool attr_set[64] = {false};                   // once per device, not per launch
@@ -621,6 +745,10 @@ int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool 
         MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false)));
         MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
         MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
+        MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             smem_bytes(false) + STOP_BYTES));
+        MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             smem_bytes(true) + STOP_BYTES));
         if (dev < 64) attr_set[dev] = true;
     }
     // rays per tile: 32 (best gather locality) unless the batch is too small to give every warpgroup a group
@@ -633,12 +761,15 @@ int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool 
     if (grid <= 0) return MVSN_OK;
     const uint8_t* w = static_cast<const uint8_t*>(wimg);
     const int smem = smem_bytes(split), nthreads = threads(split);
-    if (split) {
-        if (fast) render_wg_kernel<true, true><<<grid, nthreads, smem, stream>>>(sc, io, w);
-        else      render_wg_kernel<false, true><<<grid, nthreads, smem, stream>>>(sc, io, w);
+    if (t_stop) {                                         // early ray termination: the ray entry only
+        if (split) render_wg_kernel<true, true, true><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done);
+        else       render_wg_kernel<true, false, true><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done);
+    } else if (split) {
+        if (fast) render_wg_kernel<true, true><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
+        else      render_wg_kernel<false, true><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
     } else {
-        if (fast) render_wg_kernel<true, false><<<grid, nthreads, smem, stream>>>(sc, io, w);
-        else      render_wg_kernel<false, false><<<grid, nthreads, smem, stream>>>(sc, io, w);
+        if (fast) render_wg_kernel<true, false><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
+        else      render_wg_kernel<false, false><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
     }
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;

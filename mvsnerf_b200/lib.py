@@ -32,6 +32,7 @@ EXPORTS = [
     "mvsn_render_backward_tc_workspace_bytes", "mvsn_render_backward_tc",
     "mvsn_render_backward_deterministic_workspace_bytes", "mvsn_render_backward_deterministic",
     "mvsn_render_backward_rays_workspace_bytes", "mvsn_render_backward_rays",
+    "mvsn_render_rays_stop",
 ]
 MAX_PEERS, PEER_HANDLE_BYTES = 16, 64
 BN_BATCH, BN_BATCH_UPDATE, BN_RUNNING = 0, 1, 2
@@ -83,6 +84,9 @@ def load() -> C.CDLL:
     lib.mvsn_render_samples.argtypes = [C.POINTER(RenderScene), vp, vp, vp, vp, ip, ip, vp, vp, vp, vp, vp, vp]
     lib.mvsn_render_rays.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), vp, vp, ip, ip,
                                      vp, vp, vp, vp, vp, vp]
+    lib.mvsn_render_rays_stop.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), vp, vp, ip, ip, fp,
+                                          vp, vp, vp, vp]
+    lib.mvsn_render_rays_stop.restype = ip
     lib.mvsn_cost_volume_workspace_bytes.restype = C.c_size_t
     lib.mvsn_cost_volume_workspace_bytes.argtypes = [ip, ip, ip]
     lib.mvsn_build_cost_volume.argtypes = [vp, vp, vp, vp, ip, ip, ip, ip, ip, vp, vp, vp, C.c_size_t, vp]

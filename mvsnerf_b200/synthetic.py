@@ -125,6 +125,37 @@ def make_scene(H: int = 512, W: int = 640, pad: int = 24, seed: int = 0,
                  torch.from_numpy(c2w_t).float(), pixel_directions(H, W, focal, focal))
 
 
+def make_plane_scene(H: int = 512, W: int = 640, pad: int = 24, seed: int = 0, near_far=(2.125, 4.525),
+                     n_views: int = 3, target_shift: float = 0.1, plane=(3.0, 0.4), tex_hw=(48, 60),
+                     extent=(2.0, 1.6)) -> Scene:
+    """make_scene's cameras, but multi-view-consistent source views: each is a rendering of one textured plane
+    z = plane[0] + plane[1] * x (world frame = reference camera), between near and far.  The texture is seeded
+    uniform noise [3, *tex_hw] resampled bicubically over x in [-extent[0], extent[0]], y in [-extent[1], extent[1]].
+    The encoder recovers such geometry, so rays of the target view become opaque at the plane (make_scene's views are
+    identical images, whose only consistent depth is at infinity)."""
+    sc = make_scene(H, W, pad=pad, seed=seed, near_far=near_far, n_views=n_views, target_shift=target_shift)
+    g = torch.Generator().manual_seed(seed + 7919)
+    tex = torch.rand(1, 3, tex_hw[0], tex_hw[1], generator=g, dtype=torch.float64)
+    z0, sx = plane
+    dirs = sc.directions.reshape(-1, 3).double()                       # camera frame, z = 1
+    views = []
+    for v in range(n_views):
+        w2c = sc.pose_source["w2cs"][v].double()
+        R, t = w2c[:3, :3], w2c[:3, 3]
+        c = -R.T @ t                                                   # camera centre
+        d = dirs @ R                                                   # world directions (R^T d per row)
+        s = (z0 + sx * c[0] - c[2]) / (d[:, 2] - sx * d[:, 0])
+        p = c[None] + s[:, None] * d
+        grid = torch.stack([p[:, 0] / extent[0], p[:, 1] / extent[1]], -1).view(1, H, W, 2)
+        img = F.grid_sample(tex, grid, mode="bicubic", padding_mode="border", align_corners=True)
+        views.append(img[0].clamp(0, 1).float())
+    imgs_raw = torch.stack(views).unsqueeze(0).contiguous()          # [1,V,3,H,W]
+    mean = torch.tensor(IMAGENET_MEAN).view(1, 1, 3, 1, 1)
+    std = torch.tensor(IMAGENET_STD).view(1, 1, 3, 1, 1)
+    return Scene(H, W, pad, sc.focal, ((imgs_raw - mean) / std).contiguous(), imgs_raw, sc.proj_mats, sc.near_far,
+                 sc.pose_source, sc.c2w_target, sc.directions)
+
+
 def scene_rays(scene: Scene, c2w: torch.Tensor | None = None) -> torch.Tensor:
     c2w = scene.c2w_target if c2w is None else c2w
     return camera_rays(scene.directions, c2w, scene.near_far[0], scene.near_far[1])

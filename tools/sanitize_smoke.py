@@ -32,6 +32,14 @@ with torch.no_grad():
             sink.frame[0], sink.n_peers, sink.first_pixel = frame.data_ptr(), 1, 5
             backend.render_rays(rays, vol, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=24, mlp_mode=mode,
                                 out=(torch.empty(rays.shape[0], 3, device=dev), torch.empty(rays.shape[0], device=dev)), sink=sink)
+            if mode != lib.MLP_FP32:
+                # early ray termination (the STOP instantiations): 1994 rays x 128 samples = 499 groups of 4 rays, 8 tiles
+                # each, so CTAs hand out up to four groups through the shared counter, one CTA three (its second consumer
+                # runs idle passes), and the last group is ragged; t_stop 0 never stops, 0.5 stops some groups, 2 all
+                many = torch.cat([synthetic.scene_rays(sc)] * 2)[:1994].contiguous().to(dev)
+                for t_stop in (0.0, 0.5, 2.0):
+                    backend.render_rays(many, vol, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=128,
+                                        mlp_mode=mode, t_stop=t_stop, tiles_done=torch.zeros(1, dtype=torch.int64, device=dev))
             xyz, _, rd, z = backend.ray_marcher(rays[:100], N_samples=24)
             ndc = backend.get_ndc_coordinate(d.pose_source["w2cs"][0], d.pose_source["intrinsics"][0], xyz,
                                              torch.tensor([sc.W - 1.0, sc.H - 1.0], device=dev), near=sc.near_far[0],
