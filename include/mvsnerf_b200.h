@@ -234,6 +234,29 @@ int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const
                               const float* rays, const float* t_steps, const float* jitter, int N, int S, int grad_mode,
                               int deterministic, const mvsn_render_grads* g, float* const* grad_mlp,
                               float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream);
+/* mvsn_render_backward_rays_stop: mvsn_render_backward_rays with early ray termination.  For each ray, with alpha_j
+ * from the fp32 recompute, T_0 = 1 and T_{j+1} = T_j ((1 - alpha_j) + 1e-10) (the kernel's fp32 order), sample j is
+ * live iff T_j >= t_stop; the live samples are a prefix of length L (L >= 1).  The step renders, forms the loss of and
+ * exactly differentiates the truncated render sum_{j<L} w_j c_j (depth and white_bkgd likewise); dead samples get no
+ * gradient and no volume scatter.  Against the full render, per channel -t_stop < rgb - rgb_full <= 0 (white_bkgd:
+ * 0 <= rgb - rgb_full < t_stop) and 0 <= depth_full - depth < t_stop * far, up to a few ulps.  t_stop = 0 keeps every
+ * sample: every output is bit-identical to mvsn_render_backward_rays.  With MVSN_MLP_FP32 a ray's rgb, depth and loss
+ * term do not depend on the other rays of the batch; the MLP gradients may differ from a differently packed batch in
+ * summation order only.  deterministic != 0: every output is a deterministic function of the inputs.
+ * live_samples [N] int32 (device, 4-byte aligned, may be NULL): each ray's L.  tiles_done (device, 8-byte aligned, may
+ * be NULL): unsigned long long[3] += the 128-row tiles back-propagated immediately, deferred, and packed from deferred
+ * rays.  Everything else as mvsn_render_backward_rays.  Argument errors are returned before any CUDA call: an unknown
+ * grad_mode, NULL pointers, t_stop negative, NaN or > 1 (MVSN_EBADSHAPE), g->weights / g->alpha / g->input_feat set
+ * (MVSN_EUNSUPPORTED: per-sample cotangents of dead samples are not defined), a misaligned rays, live_samples or
+ * tiles_done, then N_samples > 128 (MVSN_EUNSUPPORTED).  Workspace: mvsn_render_backward_rays_stop_workspace_bytes(N,
+ * S, D, Hp, Wp, grad_mode, deterministic) bytes, 16-byte aligned (a little more than mvsn_render_backward_rays'). */
+size_t mvsn_render_backward_rays_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode,
+                                                      int deterministic);
+int mvsn_render_backward_rays_stop(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
+                                   const float* rays, const float* t_steps, const float* jitter, int N, int S,
+                                   int grad_mode, int deterministic, float t_stop, const mvsn_render_grads* g,
+                                   float* const* grad_mlp, float* grad_volume_dhwc, int* live_samples,
+                                   unsigned long long* tiles_done, void* workspace, size_t workspace_bytes, void* stream);
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
                    const int* numel_host, int count, float lr, float beta1, float beta2, float eps, int step,
                    void* stream);

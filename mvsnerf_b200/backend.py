@@ -730,15 +730,38 @@ def _tsteps_of(S, dev):
 
 def render_backward_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad, N_samples=128, lindisp=False,
                          jitter=None, white_bkgd=False, grads=None, target_rgb=None, n_total=None, want_volume_grad=True,
-                         grad_volume=None, grad_mlp=None, want_forward=False, loss_out=None, grad_mode=_lib.MLP_FP32):
+                         grad_volume=None, grad_mlp=None, want_forward=False, loss_out=None, grad_mode=_lib.MLP_FP32,
+                         t_stop=None, live_samples=None, tiles_done=None):
     """render_backward straight from rays [N,8] = (o, d, near, far): one mvsn_render_backward_rays launch, whose kernel
     also does ray_marcher and get_ndc_coordinate (data/ray_utils.py:152-197, utils.py:112-146) for the reference camera.
     `near_far` / `pad` / `N_samples` / `lindisp` as in render_rays.  `jitter` [N, N_samples] = perturb * u, the uniform
     draw ray_marcher makes with perturb > 0: sample s then lies at lower + (upper - lower) * jitter between the
     midpoints of its neighbours' depths, rounded as ray_marcher rounds it; None marches exactly render_rays' depths.
     Everything else, the return value and the grad_mode / torch.use_deterministic_algorithms dispatch are as in
-    render_backward (the depth the `grads` dict differentiates is the jittered one)."""
+    render_backward (the depth the `grads` dict differentiates is the jittered one).
+
+    `t_stop` (a float in [0, 1]): early ray termination (mvsn_render_backward_rays_stop) -- each ray keeps the prefix of
+    samples whose transmittance in front of them is >= t_stop, and the step renders, forms the loss of and exactly
+    differentiates that truncated render; each channel differs from the full render by less than t_stop (t_stop = 0:
+    bit-identical to t_stop=None).  Per-sample cotangents (`grads` 'weights', 'alpha', 'input_feat') are rejected with
+    it.  `live_samples`: an optional CUDA int32 tensor [N] that receives each ray's number of kept samples;
+    `tiles_done`: an optional CUDA int64 tensor [3] the counts of tiles back-propagated immediately, deferred and packed
+    are added to."""
     _check_grad_mode(grad_mode)
+    if t_stop is not None:
+        t_stop = float(t_stop)
+        if not 0.0 <= t_stop <= 1.0:
+            raise RuntimeError(f"render_backward_rays: t_stop={t_stop} must be in [0, 1]")
+        if grads is not None and any(grads.get(k) is not None for k in ("weights", "alpha", "input_feat")):
+            raise RuntimeError("render_backward_rays: t_stop takes no per-sample cotangents (weights / alpha / input_feat):"
+                               " dead samples have none")
+        for t, name, dtype, n in ((live_samples, "live_samples", torch.int32, rays.shape[0]), (tiles_done, "tiles_done", torch.int64, 3)):
+            if t is not None and (not t.is_cuda or t.device != rays.device or t.dtype != dtype or t.numel() < n
+                                  or not t.is_contiguous()):
+                raise RuntimeError(f"render_backward_rays: {name} must be a contiguous CUDA {dtype} tensor of >= {n} "
+                                   f"elements on the rays' device ({rays.device})")
+    elif live_samples is not None or tiles_done is not None:
+        raise RuntimeError("render_backward_rays: live_samples / tiles_done need t_stop")
     lib = _lib.load()
     rays = _lib.dev_f32(rays.detach(), "rays")
     N, S = rays.shape[0], int(N_samples)
@@ -757,19 +780,26 @@ def render_backward_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_
     g, held, rgb, depth = _render_grads(N, S, dev, grads, target_rgb, n_total, want_forward, loss_out)
     det = torch.are_deterministic_algorithms_enabled()
     dims = (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0)
-    need = lib.mvsn_render_backward_rays_workspace_bytes(N, S, *dims, int(grad_mode), int(det))
+    ws_bytes = (lib.mvsn_render_backward_rays_workspace_bytes if t_stop is None
+                else lib.mvsn_render_backward_rays_stop_workspace_bytes)
+    need = ws_bytes(N, S, *dims, int(grad_mode), int(det))
     if need == 0:
         raise RuntimeError(f"render_backward_rays: unsupported shape N={N}, N_samples={S} (N_samples <= 128)")
     ws = _bwd_workspace.get(dev)
     if ws is None or ws.numel() < need:
         ws = torch.empty(need, dtype=torch.uint8, device=dev)
         _bwd_workspace[dev] = ws
+    head = (C.byref(sc), _lib.ptr_array(params), C.byref(rp), _lib.ptr(rays), _lib.ptr(_tsteps_of(S, dev)),
+            _lib.ptr(jitter), N, S, int(grad_mode), int(det))
+    tail = (C.byref(g), _lib.ptr_array(grad_mlp), _lib.ptr(grad_volume) if want_volume_grad else None)
     with torch.cuda.device(dev):
-        _lib.check(lib.mvsn_render_backward_rays(
-            C.byref(sc), _lib.ptr_array(params), C.byref(rp), _lib.ptr(rays), _lib.ptr(_tsteps_of(S, dev)),
-            _lib.ptr(jitter), N, S, int(grad_mode), int(det), C.byref(g), _lib.ptr_array(grad_mlp),
-            _lib.ptr(grad_volume) if want_volume_grad else None, _lib.ptr(ws), need, _lib.stream_ptr()),
-            "mvsn_render_backward_rays")
+        if t_stop is None:
+            _lib.check(lib.mvsn_render_backward_rays(*head, *tail, _lib.ptr(ws), need, _lib.stream_ptr()),
+                       "mvsn_render_backward_rays")
+        else:
+            _lib.check(lib.mvsn_render_backward_rays_stop(*head, t_stop, *tail, _lib.ptr(live_samples),
+                                                          _lib.ptr(tiles_done), _lib.ptr(ws), need, _lib.stream_ptr()),
+                       "mvsn_render_backward_rays_stop")
     del keep, held
     return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
 
@@ -832,13 +862,14 @@ class FineTuner:
         return self.loss, (rgb, depth)
 
     def step_rays(self, rays, target_rgb, near_far, pad, N_samples=128, lindisp=False, perturb=1.0, generator=None,
-                  lr=None, want_forward=False):
+                  lr=None, want_forward=False, t_stop=None):
         """One optimisation step on a batch of rays [N,8] = (o, d, near, far), as train_mvs_nerf_finetuning_pl.py:140-164
         feeds it: the ray march (ray_marcher with `perturb`) and the NDC conversion run inside the backward kernel
         (render_backward_rays).  With perturb > 0 the jitter is drawn as ray_marcher draws it, `perturb *
         torch.rand((N, N_samples))` (from `generator`, or the default generator), so switching a run from
         `step(*ray_marcher(...))` to step_rays consumes the same random stream.  `near_far` / `pad` as in render_rays.
-        Returns what `step` returns."""
+        `t_stop`: early ray termination, as in render_backward_rays -- the step trains the render truncated where each
+        ray's transmittance falls below t_stop, and skips the work of the samples behind.  Returns what `step` returns."""
         lr = self.lr if lr is None else float(lr)
         rays = _lib.dev_f32(rays.detach(), "rays")
         jitter = None
@@ -850,7 +881,7 @@ class FineTuner:
                                                 pad, N_samples=N_samples, lindisp=lindisp, jitter=jitter,
                                                 white_bkgd=self.white_bkgd, target_rgb=target_rgb, want_volume_grad=True,
                                                 grad_volume=self.vol_g, grad_mlp=self.g, want_forward=want_forward,
-                                                loss_out=self.loss, grad_mode=self.grad_mode)
+                                                loss_out=self.loss, grad_mode=self.grad_mode, t_stop=t_stop)
         self._adam(lr)
         return self.loss, (rgb, depth)
 

@@ -410,27 +410,41 @@ size_t mvsn_render_backward_rays_workspace_bytes(int N, int S, int D, int Hp, in
     return tc ? render_backward_tc_workspace_bytes(N, S) : render_backward_workspace_bytes(N, S);
 }
 
-int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
-                              const float* rays, const float* t_steps, const float* jitter, int N, int S, int grad_mode,
-                              int deterministic, const mvsn_render_grads* g, float* const* grad_mlp,
-                              float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream) {
-    MVSN_RANGE("mvsn_render_backward_rays");
+// mvsn_render_backward_rays and, with `stop`, mvsn_render_backward_rays_stop (`what`: the entry's name for messages)
+static int backward_rays_entry(const char* what, const mvsn_render_scene* scene, const float* const* mlp_w,
+                               const mvsn_ray_params* rp, const float* rays, const float* t_steps, const float* jitter,
+                               int N, int S, int grad_mode, int deterministic, const mvsn_render_grads* g,
+                               float* const* grad_mlp, float* grad_volume_dhwc, void* workspace, size_t workspace_bytes,
+                               void* stream, const BwdStop* stop) {
     MVSN_REQUIRE(grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF, MVSN_EUNSUPPORTED,
-                 "mvsn_render_backward_rays: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)", grad_mode);
+                 "%s: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)", what, grad_mode);
     SceneDev sc;
     int rc = make_scene(scene, sc);
     if (rc) return rc;
-    MVSN_REQUIRE(rp && g && mlp_w && grad_mlp, MVSN_ENULL, "mvsn_render_backward_rays: NULL argument");
-    MVSN_REQUIRE(g->rgb || g->target_rgb, MVSN_ENULL, "mvsn_render_backward_rays: neither g->rgb nor g->target_rgb given");
+    MVSN_REQUIRE(rp && g && mlp_w && grad_mlp, MVSN_ENULL, "%s: NULL argument", what);
+    MVSN_REQUIRE(g->rgb || g->target_rgb, MVSN_ENULL, "%s: neither g->rgb nor g->target_rgb given", what);
     for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i)
-        MVSN_REQUIRE(mlp_w[i] && grad_mlp[i], MVSN_ENULL, "mvsn_render_backward_rays: tensor %d is NULL", i);
-    MVSN_REQUIRE(N == 0 || (rays && t_steps), MVSN_ENULL, "mvsn_render_backward_rays: rays or t_steps is NULL");
-    MVSN_REQUIRE(aligned16(rays), MVSN_EALIGN, "mvsn_render_backward_rays: rays must be 16-byte aligned");
+        MVSN_REQUIRE(mlp_w[i] && grad_mlp[i], MVSN_ENULL, "%s: tensor %d is NULL", what, i);
+    MVSN_REQUIRE(N == 0 || (rays && t_steps), MVSN_ENULL, "%s: rays or t_steps is NULL", what);
+    if (stop) {
+        MVSN_REQUIRE(stop->t_stop >= 0.f && stop->t_stop <= 1.f, MVSN_EBADSHAPE,
+                     "%s: t_stop=%g must be in [0, 1] (not NaN)", what, (double)stop->t_stop);
+        MVSN_REQUIRE(!g->weights && !g->alpha && !g->input_feat, MVSN_EUNSUPPORTED,
+                     "%s: g->weights / g->alpha / g->input_feat are per-sample cotangents, not defined for dead samples",
+                     what);
+    }
+    MVSN_REQUIRE(aligned16(rays), MVSN_EALIGN, "%s: rays must be 16-byte aligned", what);
     MVSN_REQUIRE(!grad_volume_dhwc || aligned16(grad_volume_dhwc), MVSN_EALIGN, "grad_volume_dhwc must be 16-byte aligned");
-    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "mvsn_render_backward_rays: N=%d S=%d", N, S);
-    MVSN_REQUIRE(S <= 128, MVSN_EUNSUPPORTED, "mvsn_render_backward_rays: N_samples=%d > 128 is not implemented", S);
+    if (stop) {
+        MVSN_REQUIRE(reinterpret_cast<uintptr_t>(stop->live_samples) % 4 == 0, MVSN_EALIGN,
+                     "%s: live_samples must be 4-byte aligned", what);
+        MVSN_REQUIRE(reinterpret_cast<uintptr_t>(stop->tiles_done) % 8 == 0, MVSN_EALIGN,
+                     "%s: tiles_done must be 8-byte aligned", what);
+    }
+    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "%s: N=%d S=%d", what, N, S);
+    MVSN_REQUIRE(S <= 128, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, S);
     MVSN_REQUIRE(scene->mlp_mode == MVSN_MLP_FP32, MVSN_EUNSUPPORTED,
-                 "mvsn_render_backward_rays: scene->mlp_packed must be the MVSN_MLP_FP32 image (mode %d given)", scene->mlp_mode);
+                 "%s: scene->mlp_packed must be the MVSN_MLP_FP32 image (mode %d given)", what, scene->mlp_mode);
     if (N == 0) return MVSN_OK;
     RenderIO io{};
     io.rays = rays; io.t_steps = t_steps;
@@ -439,7 +453,32 @@ int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const
     return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
                                   g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
                                   grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
-                                  (cudaStream_t)stream, grad_mode == MVSN_MLP_TC_HALF, deterministic != 0, jitter);
+                                  (cudaStream_t)stream, grad_mode == MVSN_MLP_TC_HALF, deterministic != 0, jitter, stop);
+}
+
+int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
+                              const float* rays, const float* t_steps, const float* jitter, int N, int S, int grad_mode,
+                              int deterministic, const mvsn_render_grads* g, float* const* grad_mlp,
+                              float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward_rays");
+    return backward_rays_entry("mvsn_render_backward_rays", scene, mlp_w, rp, rays, t_steps, jitter, N, S, grad_mode,
+                               deterministic, g, grad_mlp, grad_volume_dhwc, workspace, workspace_bytes, stream, nullptr);
+}
+
+size_t mvsn_render_backward_rays_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
+    if (grad_mode != MVSN_MLP_FP32 && grad_mode != MVSN_MLP_TC_HALF) return 0;
+    return render_backward_stop_workspace_bytes(N, S, D, Hp, Wp, grad_mode == MVSN_MLP_TC_HALF, deterministic != 0);
+}
+
+int mvsn_render_backward_rays_stop(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
+                                   const float* rays, const float* t_steps, const float* jitter, int N, int S,
+                                   int grad_mode, int deterministic, float t_stop, const mvsn_render_grads* g,
+                                   float* const* grad_mlp, float* grad_volume_dhwc, int* live_samples,
+                                   unsigned long long* tiles_done, void* workspace, size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward_rays_stop");
+    const BwdStop stop{t_stop, live_samples, tiles_done};
+    return backward_rays_entry("mvsn_render_backward_rays_stop", scene, mlp_w, rp, rays, t_steps, jitter, N, S, grad_mode,
+                               deterministic, g, grad_mlp, grad_volume_dhwc, workspace, workspace_bytes, stream, &stop);
 }
 
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,

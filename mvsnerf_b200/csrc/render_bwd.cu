@@ -102,6 +102,15 @@ struct DetIO {
     unsigned* amax;          // [2] max |g| over the finite recorded values (float bits), and a non-finite flag
 };
 
+// What the STOP = true kernels (mvsn_render_backward_rays_stop) take besides
+struct StopIO {
+    float t_stop;                    // sample j of a ray is live iff its transmittance T_j >= t_stop
+    int* live;                       // [N] live samples per ray (the caller's live_samples, or the workspace)
+    int2* list;                      // per CTA: list_cap (ray, live samples) entries deferred to phase B
+    int list_cap;
+    unsigned long long* tiles_done;  // [3] += tiles back-propagated immediately, deferred, packed (may be null)
+};
+
 namespace {
 
 // fragment <-> memory helpers of the backward (fragment layout: frag_row / frag_col in tile_fp32.cuh)
@@ -176,34 +185,181 @@ constexpr int BWD_SMEM_FLOATS = TILE_SMEM_FLOATS + TILE_M * 18;
 constexpr size_t BWD_SMEM_BYTES = BWD_SMEM_FLOATS * sizeof(float);
 static_assert(TILE_M * PE_LD >= 64 * H_LD, "peT staging [64][H_LD] must fit in the positional-encoding region");
 
+// ---- early ray termination (STOP = true, mvsn_render_backward_rays_stop) -----------------------------------------
+// Sample j of a ray is live iff T_j >= t_stop (T_0 = 1, T_{j+1} = T_j ((1 - alpha_j) + 1e-10), the scan's fp32 order);
+// T never increases, so the live samples are a prefix of length L.  The kernel differentiates exactly the truncated
+// render sum_{j<L} w_j c_j: dead samples get s_g = 0 and no volume scatter.  Two phases in the persistent launch:
+//   A  the CTA's static groups, as the other kernels take them.  After the forward scan the tile is back-propagated
+//      at once (dead rows zero: every GEMM, column sum and scatter is linear in s_g) unless some of its samples are
+//      dead and fewer than TILE_M / 2 rows are live; then its rays (ray, L) are appended to the CTA's list instead.
+//   B  the CTA's listed rays, in list order and whole, packed into 128-row tiles, recomputed and back-propagated.
+// The tile's rows and rays come from tables in shared memory behind the backward's own (StopTables); the forward
+// tile, the GEMMs and the heads do not care which rows they hold.  A sample's forward is its own row's (fp32, row-
+// independent), so its alpha, and the ray's L, are the same in both phases; rgb / depth / the loss are written in
+// phase A only.
+namespace stopt {
+constexpr int ROW_SLOT = 0;                  // [128] row -> ray slot of the tile, -1: empty row
+constexpr int ROW_S    = ROW_SLOT + TILE_M;  // [128] row -> sample index in its ray
+constexpr int RAY      = ROW_S + TILE_M;     // [128] slot -> ray (-1: past N)
+constexpr int FIRST    = RAY + TILE_M;       // [128] slot -> first row
+constexpr int LEN      = FIRST + TILE_M;     // [128] slot -> rows (after the scan: live samples)
+constexpr int MISC     = LEN + TILE_M;
+enum { N_RAYS, N_ROWS, LIVE_ROWS, PHASE_B, N_LIST, CURSOR, N_IMM, N_DEF, N_PACKED, N_MISC };
+constexpr int INTS     = MISC + N_MISC;
+}  // namespace stopt
+constexpr size_t STOP_SMEM_BYTES = stopt::INTS * sizeof(int);
+
+struct StopTables {
+    int* t;
+    __device__ __forceinline__ explicit StopTables(float* smem) : t(reinterpret_cast<int*>(smem + BWD_SMEM_FLOATS)) {}
+    __device__ __forceinline__ int& misc(int i) const { return t[stopt::MISC + i]; }
+};
+
+// phase A: group grp in the standard mapping (slot r = ray grp * R + r, rows [r S, r S + S))
+__device__ __forceinline__ void stop_plan_group(const StopTables& st, int grp, int R, int S, int N, int tid) {
+    if (tid < TILE_M) {
+        const int r_in = tid / S;
+        st.t[stopt::ROW_SLOT + tid] = r_in < R && grp * R + r_in < N ? r_in : -1;
+        st.t[stopt::ROW_S + tid] = tid - r_in * S;
+    }
+    if (tid < R) {
+        const int ray = grp * R + tid;
+        st.t[stopt::RAY + tid] = ray < N ? ray : -1;
+        st.t[stopt::FIRST + tid] = tid * S;
+        st.t[stopt::LEN + tid] = S;
+    }
+    if (tid == 0) { st.misc(stopt::N_RAYS) = R; st.misc(stopt::N_ROWS) = R * S; st.misc(stopt::LIVE_ROWS) = 0; }
+}
+
+// phase B, one thread: the next packed tile from the CTA's list (N_RAYS = 0: the list is done)
+__device__ __forceinline__ void stop_pack_tile(const StopTables& st, const int2* list) {
+    int c = st.misc(stopt::CURSOR), rows = 0, k = 0;
+    const int n = st.misc(stopt::N_LIST);
+    for (; c < n; ++c, ++k) {
+        const int2 e = list[c];                              // e.y >= 1: T_0 = 1 >= t_stop
+        if (rows + e.y > TILE_M) break;
+        st.t[stopt::RAY + k] = e.x; st.t[stopt::FIRST + k] = rows; st.t[stopt::LEN + k] = e.y;
+        for (int s = 0; s < e.y; ++s) { st.t[stopt::ROW_SLOT + rows + s] = k; st.t[stopt::ROW_S + rows + s] = s; }
+        rows += e.y;
+    }
+    for (int r = rows; r < TILE_M; ++r) { st.t[stopt::ROW_SLOT + r] = -1; st.t[stopt::ROW_S + r] = 0; }
+    st.misc(stopt::CURSOR) = c; st.misc(stopt::N_RAYS) = k; st.misc(stopt::N_ROWS) = rows;
+    st.misc(stopt::LIVE_ROWS) = 0; st.misc(stopt::PHASE_B) = 1;
+    if (k) ++st.misc(stopt::N_PACKED);
+}
+
+// Top of a tile: the tables of phase A's group grp, or of phase B's next packed tile.  False: nothing left.
+__device__ __forceinline__ bool stop_next_tile(float* smem, const StopIO& stop, int grp, int ngroups, int R, int S, int N,
+                                               int tid) {
+    const StopTables st(smem);
+    if (grp < ngroups) stop_plan_group(st, grp, R, S, N, tid);
+    else if (tid == 0) stop_pack_tile(st, stop.list + (size_t)blockIdx.x * stop.list_cap);
+    __syncthreads();
+    return st.misc(stopt::N_RAYS) != 0;
+}
+
+// Row tid of the tile (tid < TILE_M): its ray and sample; false for an empty row
+__device__ __forceinline__ bool stop_row(float* smem, int tid, int& ray, int& s_idx) {
+    const StopTables st(smem);
+    const int slot = st.t[stopt::ROW_SLOT + tid];
+    s_idx = st.t[stopt::ROW_S + tid];
+    ray = slot >= 0 ? st.t[stopt::RAY + slot] : 0;
+    return slot >= 0;
+}
+
+// After the forward scan: whether row tid holds a live sample (the rows the volume scatter takes)
+__device__ __forceinline__ bool stop_row_live(float* smem, int tid) {
+    const StopTables st(smem);
+    const int slot = st.t[stopt::ROW_SLOT + tid];
+    return slot >= 0 && st.t[stopt::ROW_S + tid] < st.t[stopt::LEN + slot];
+}
+
+// Phase A, after the forward scan and a barrier: defer the tile (append its rays to the CTA's list) or back-propagate
+// it now.  A tile none of whose samples is dead is never deferred, so t_stop = 0 does exactly the work of the kernels
+// without STOP.  Ends with a barrier (every thread has read the counters thread 0 then updates).
+__device__ __forceinline__ bool stop_defer(float* smem, const StopIO& stop, int grp, int ngroups, int R, int S, int N,
+                                           int tid) {
+    const StopTables st(smem);
+    if (grp >= ngroups) return false;                          // a packed tile (phase B)
+    const int nvalid = min(R, N - grp * R), live = st.misc(stopt::LIVE_ROWS);
+    const bool defer = live < nvalid * S && 2 * live < TILE_M;
+    if (defer && tid < nvalid)
+        stop.list[(size_t)blockIdx.x * stop.list_cap + st.misc(stopt::N_LIST) + tid] =
+            make_int2(st.t[stopt::RAY + tid], st.t[stopt::LEN + tid]);
+    __syncthreads();
+    if (tid == 0) {
+        if (defer) { st.misc(stopt::N_LIST) += nvalid; ++st.misc(stopt::N_DEF); }
+        else ++st.misc(stopt::N_IMM);
+    }
+    return defer;
+}
+
+__device__ __forceinline__ void stop_init(float* smem, int tid) {
+    if (tid < stopt::N_MISC) StopTables(smem).misc(tid) = 0;
+}
+
+__device__ __forceinline__ void stop_finish(float* smem, const StopIO& stop, int tid) {
+    const StopTables st(smem);
+    if (tid == 0 && stop.tiles_done) {
+        atomicAdd(stop.tiles_done, (unsigned long long)st.misc(stopt::N_IMM));
+        atomicAdd(stop.tiles_done + 1, (unsigned long long)st.misc(stopt::N_DEF));
+        atomicAdd(stop.tiles_done + 2, (unsigned long long)st.misc(stopt::N_PACKED));
+    }
+}
+
 // Compositing of a tile, forward and reverse scan, one thread per ray (renderer.py:65-92).  Writes rgb_out /
 // depth_out / the fused loss, s_T (transmittance in front of each sample) and s_g (d rgb_pre, d sigma_pre per row).
 // f_j = 1 - alpha_j + 1e-10, T_{j+1} = T_j f_j, w_j = alpha_j T_j.
 // d alpha_j = T_j (d w_j - B_j),  B_{j-1} = d w_j alpha_j + f_j B_j  (no division by f_j).
 // DET: the ray's loss term goes to det.loss_terms[ray] instead of being added to bw.loss.
-template <bool DET>
+// STOP: the rays and rows come from the StopTables; the forward stops at the first dead sample (T_j < t_stop), the
+// ray's live count L goes to the table (LEN) and, in phase A, to stop->live; the dead rows get s_g = 0; rgb_out /
+// depth_out / the loss are written in phase A only.
+template <bool DET, bool STOP = false>
 __device__ __forceinline__ void composite_scan(const SceneDev& sc, const BwdIO& bw, const TileSmem& sm, float* s_T, float* s_g,
-                                               int grp, int R, int S, int N, int tid, const DetIO& det) {
-    if (tid < R) {
-        const int ray = grp * R + tid, first = tid * S;
-        if (ray < N) {
+                                               int grp, int R, int S, int N, int tid, const DetIO& det,
+                                               const StopIO* stop = nullptr, float* smem = nullptr) {
+    int nrays = R, nrows = R * S;
+    bool emit = true;
+    if constexpr (STOP) {
+        const StopTables st(smem);
+        nrays = st.misc(stopt::N_RAYS); nrows = st.misc(stopt::N_ROWS); emit = st.misc(stopt::PHASE_B) == 0;
+    }
+    if (tid < nrays) {
+        int ray = grp * R + tid, first = tid * S, len = S;
+        bool ok = ray < N;
+        if constexpr (STOP) {
+            const StopTables st(smem);
+            ray = st.t[stopt::RAY + tid]; first = st.t[stopt::FIRST + tid]; len = st.t[stopt::LEN + tid]; ok = ray >= 0;
+        }
+        if (ok) {
             float cr = 0.f, cg = 0.f, cb = 0.f, dp = 0.f, ac = 0.f, T = 1.f;
-            for (int j = first; j < first + S; ++j) {
+            int end = first + len;
+            for (int j = first; j < first + len; ++j) {
+                if constexpr (STOP) { if (T < stop->t_stop) { end = j; break; } }
                 const float a = sm.rgb[j * 4 + 3], w = a * T;
                 s_T[j] = T;
                 cr = fmaf(w, sm.rgb[j * 4 + 0], cr); cg = fmaf(w, sm.rgb[j * 4 + 1], cg); cb = fmaf(w, sm.rgb[j * 4 + 2], cb);
                 dp = fmaf(w, sm.z[j], dp); ac += w;
                 T *= (1.f - a) + 1e-10f;
             }
+            if constexpr (STOP) {
+                const StopTables st(smem);
+                const int L = end - first;
+                for (int j = end; j < first + len; ++j) { s_g[j * 4] = s_g[j * 4 + 1] = s_g[j * 4 + 2] = s_g[j * 4 + 3] = 0.f; }
+                st.t[stopt::LEN + tid] = L;
+                if (emit) stop->live[ray] = L;
+                atomicAdd(&st.misc(stopt::LIVE_ROWS), L);
+            }
             if (sc.white_bkgd) { const float bg = 1.f - ac; cr += bg; cg += bg; cb += bg; }
-            if (bw.rgb_out) { bw.rgb_out[(size_t)ray * 3] = cr; bw.rgb_out[(size_t)ray * 3 + 1] = cg; bw.rgb_out[(size_t)ray * 3 + 2] = cb; }
-            if (bw.depth_out) bw.depth_out[ray] = dp;
+            if (emit && bw.rgb_out) { bw.rgb_out[(size_t)ray * 3] = cr; bw.rgb_out[(size_t)ray * 3 + 1] = cg; bw.rgb_out[(size_t)ray * 3 + 2] = cb; }
+            if (emit && bw.depth_out) bw.depth_out[ray] = dp;
             float g0, g1, g2;
             if (bw.target) {                     // fused img2mse (utils.py: mean((rgb - target)^2))
                 const float e0 = cr - __ldg(bw.target + (size_t)ray * 3), e1 = cg - __ldg(bw.target + (size_t)ray * 3 + 1),
                             e2 = cb - __ldg(bw.target + (size_t)ray * 3 + 2);
                 g0 = 2.f * e0 * bw.inv_count; g1 = 2.f * e1 * bw.inv_count; g2 = 2.f * e2 * bw.inv_count;
-                if (bw.loss) {
+                if (emit && bw.loss) {
                     if constexpr (DET) det.loss_terms[ray] = (e0 * e0 + e1 * e1 + e2 * e2) * bw.inv_count;
                     else               atomicAdd(bw.loss, (e0 * e0 + e1 * e1 + e2 * e2) * bw.inv_count);
                 }
@@ -213,7 +369,7 @@ __device__ __forceinline__ void composite_scan(const SceneDev& sc, const BwdIO& 
             const float gd = bw.g_depth ? __ldg(bw.g_depth + ray) : 0.f;
             const float gbg = sc.white_bkgd ? (g0 + g1 + g2) : 0.f;
             float B = 0.f;
-            for (int j = first + S - 1; j >= first; --j) {
+            for (int j = end - 1; j >= first; --j) {
                 const size_t sj = (size_t)ray * S + (j - first);
                 const float a = sm.rgb[j * 4 + 3], Tj = s_T[j], w = a * Tj;
                 const float c0 = sm.rgb[j * 4], c1 = sm.rgb[j * 4 + 1], c2 = sm.rgb[j * 4 + 2];
@@ -228,10 +384,10 @@ __device__ __forceinline__ void composite_scan(const SceneDev& sc, const BwdIO& 
                 s_g[j * 4 + 3] = sm.sig[j] > 0.f ? da * (1.f - a) : 0.f;
             }
         } else {
-            for (int j = first; j < first + S; ++j) { s_g[j * 4] = s_g[j * 4 + 1] = s_g[j * 4 + 2] = s_g[j * 4 + 3] = 0.f; }
+            for (int j = first; j < first + len; ++j) { s_g[j * 4] = s_g[j * 4 + 1] = s_g[j * 4 + 2] = s_g[j * 4 + 3] = 0.f; }
         }
     }
-    if (tid >= R * S && tid < TILE_M) { s_g[tid * 4] = s_g[tid * 4 + 1] = s_g[tid * 4 + 2] = s_g[tid * 4 + 3] = 0.f; }
+    if (tid >= nrows && tid < TILE_M) { s_g[tid * 4] = s_g[tid * 4 + 1] = s_g[tid * 4 + 2] = s_g[tid * 4 + 3] = 0.f; }
 }
 
 // Element-wise stage of trunk layer l on the thread's fragment: acc = d h_{l+1}  ->  d g = acc * (h > 0) ;
@@ -318,10 +474,12 @@ __device__ __forceinline__ void volume_scatter(const SceneDev& sc, const RenderI
 
 // FAST: the front end marches the samples from io.rays / io.t_steps (stratified by `jitter` [N,S] unless NULL) instead of
 // reading io.pts / io.ndc / io.z / io.dirs (mvsn_render_backward_rays); `jitter` is unused otherwise.
-template <bool DET, bool FAST>
+// STOP (FAST only): early ray termination at stop.t_stop, in two phases (described above StopTables); the launch adds
+// STOP_SMEM_BYTES of dynamic shared memory for the tables.  `stop` is unused otherwise.
+template <bool DET, bool FAST, bool STOP = false>
 __global__ void __launch_bounds__(256, 1)
 render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts, const DetIO det,
-                  const float* __restrict__ jitter) {
+                  const float* __restrict__ jitter, const StopIO stop) {
     extern __shared__ __align__(16) float smem[];
     const TileSmem sm(smem);                       // backward: sm.pe holds peT as [64][H_LD]; sm.h, sm.mod the A operands
     float* s_T    = sm.tail;                       // [128] transmittance in front of the sample
@@ -335,28 +493,42 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
     float* G = bw.grads + (size_t)blockIdx.x * bwd::GRADS;
     for (int i = tid; i < bwd::GRADS; i += 256) G[i] = 0.f;
     for (int i = tid; i < 32 * 128; i += 256) scr[bwd::S_FEATT + 32 * 128 + i] = 0.f;      // featT rows 32..63 stay zero
+    if constexpr (STOP) stop_init(smem, tid);
     __syncthreads();
 
     const int N = io.N, S = io.S;
     const int R = TILE_M / S;                                   // rays per tile (S <= 128, checked by the launcher)
     const int ngroups = (N + R - 1) / R;
 
-    for (int grp = blockIdx.x; grp < ngroups; grp += gridDim.x) {
+    // STOP: phase A's groups, then phase B's packed tiles (grp >= ngroups) until the CTA's list is done
+    for (int grp = blockIdx.x; STOP || grp < ngroups; grp += gridDim.x) {
+        if constexpr (STOP) { if (!stop_next_tile(smem, stop, grp, ngroups, R, S, N, tid)) break; }
         // =============================== forward recompute ===========================================
         bool valid = false;
         size_t si = 0;
         if (tid < TILE_M) {
-            const int r_in = tid / S, s_idx = tid - r_in * S, ray = grp * R + r_in;
-            valid = r_in < R && ray < N;
-            si = (size_t)ray * S + s_idx;
-            tile_front_end<FAST>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr}, jitter);
+            if constexpr (STOP) {
+                int ray, s_idx;
+                valid = stop_row(smem, tid, ray, s_idx);
+                si = (size_t)ray * S + s_idx;
+                tile_front_end<FAST>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr}, jitter);
+            } else {
+                const int r_in = tid / S, s_idx = tid - r_in * S, ray = grp * R + r_in;
+                valid = r_in < R && ray < N;
+                si = (size_t)ray * S + s_idx;
+                tile_front_end<FAST>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr}, jitter);
+            }
         }
         __syncthreads();
         tile_mlp(sm, wts, tid, ScratchRecord{scr});
         __syncthreads();
 
         // =============================== compositing: forward + reverse scan ===========================
-        composite_scan<DET>(sc, bw, sm, s_T, s_g, grp, R, S, N, tid, det);
+        composite_scan<DET, STOP>(sc, bw, sm, s_T, s_g, grp, R, S, N, tid, det, &stop, smem);
+        if constexpr (STOP) {
+            __syncthreads();                                    // every ray's live count
+            if (stop_defer(smem, stop, grp, ngroups, R, S, N, tid)) continue;
+        }
         stage_T(sm.pe, scr + bwd::S_PET, 64, tid);             // peT -> shared (used by the layer-5 and layer-0 wgrads)
         __syncthreads();
 
@@ -498,10 +670,12 @@ render_bwd_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const fl
                     *reinterpret_cast<float4*>(s_df + frag_row(ty, r) * 8 + tx * 4) = make_float4(a[r][0], a[r][1], a[r][2], a[r][3]);
             }
             __syncthreads();
-            if (tid < TILE_M && valid) volume_scatter<DET, FAST>(sc, io, bw, s_df, si, tid, det, scr);   // trilinear scatter
+            if constexpr (STOP) { if (tid < TILE_M && stop_row_live(smem, tid)) volume_scatter<DET, FAST>(sc, io, bw, s_df, si, tid, det, scr); }
+            else if (tid < TILE_M && valid) volume_scatter<DET, FAST>(sc, io, bw, s_df, si, tid, det, scr);   // trilinear scatter
         }
         __syncthreads();
     }
+    if constexpr (STOP) stop_finish(smem, stop, tid);
 }
 
 // ---- per-CTA accumulators -> the 22 tensors in nn.Linear layout ---------------------------------------------
@@ -750,10 +924,10 @@ __device__ __forceinline__ void frag_load_rm(float (&acc)[8][8], const float* sr
     __syncthreads();
 }
 
-template <bool DET, bool FAST>
+template <bool DET, bool FAST, bool STOP = false>
 __global__ void __launch_bounds__(256, 1)
 render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts,
-                     const __half* __restrict__ wh, const DetIO det, const float* __restrict__ jitter) {
+                     const __half* __restrict__ wh, const DetIO det, const float* __restrict__ jitter, const StopIO stop) {
     using namespace bwdtc;
     extern __shared__ __align__(16) float smem[];
     const TileSmem sm(smem);
@@ -775,26 +949,39 @@ render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const
     float* G = bw.grads + (size_t)blockIdx.x * bwd::GRADS;
     for (int i = tid; i < bwd::GRADS; i += 256) G[i] = 0.f;
     for (int i = tid; i < 32 * 128; i += 256) scr[bwd::S_FEATT + 32 * 128 + i] = 0.f;
+    if constexpr (STOP) stop_init(smem, tid);
     __syncthreads();
 
     const int N = io.N, S = io.S;
     const int R = TILE_M / S;
     const int ngroups = (N + R - 1) / R;
 
-    for (int grp = blockIdx.x; grp < ngroups; grp += gridDim.x) {
+    for (int grp = blockIdx.x; STOP || grp < ngroups; grp += gridDim.x) {
+        if constexpr (STOP) { if (!stop_next_tile(smem, stop, grp, ngroups, R, S, N, tid)) break; }
         // =============================== forward recompute (the fp32 tile) ===========================
         bool valid = false;
         size_t si = 0;
         if (tid < TILE_M) {
-            const int r_in = tid / S, s_idx = tid - r_in * S, ray = grp * R + r_in;
-            valid = r_in < R && ray < N;
-            si = (size_t)ray * S + s_idx;
-            tile_front_end<FAST>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr}, jitter);
+            if constexpr (STOP) {
+                int ray, s_idx;
+                valid = stop_row(smem, tid, ray, s_idx);
+                si = (size_t)ray * S + s_idx;
+                tile_front_end<FAST>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr}, jitter);
+            } else {
+                const int r_in = tid / S, s_idx = tid - r_in * S, ray = grp * R + r_in;
+                valid = r_in < R && ray < N;
+                si = (size_t)ray * S + s_idx;
+                tile_front_end<FAST>(sc, cams, io, sm, tid, ray, s_idx, valid, ScratchRecord{scr}, jitter);
+            }
         }
         __syncthreads();
         tile_mlp(sm, wts, tid, ScratchRecord{scr});
         __syncthreads();
-        composite_scan<DET>(sc, bw, sm, s_T, s_g, grp, R, S, N, tid, det);
+        composite_scan<DET, STOP>(sc, bw, sm, s_T, s_g, grp, R, S, N, tid, det, &stop, smem);
+        if constexpr (STOP) {
+            __syncthreads();
+            if (stop_defer(smem, stop, grp, ngroups, R, S, N, tid)) continue;
+        }
         load_w_issue(wh + W_VF, 64 * 128, w16, tid);
         __syncthreads();
         const int e_pe = stage_half(scr + bwd::S_PET, 128, 64, 128, pe16, s_amax, amax_i, tid);
@@ -938,10 +1125,12 @@ render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const
                 *reinterpret_cast<float2*>(s_df + (64 * wg + 16 * w + g + 8 * hh) * 8 + 2 * q) =
                     make_float2(d1[0][2 * hh] * sc_m, d1[0][2 * hh + 1] * sc_m);
             __syncthreads();
-            if (tid < TILE_M && valid) volume_scatter<DET, FAST>(sc, io, bw, s_df, si, tid, det, scr);
+            if constexpr (STOP) { if (tid < TILE_M && stop_row_live(smem, tid)) volume_scatter<DET, FAST>(sc, io, bw, s_df, si, tid, det, scr); }
+            else if (tid < TILE_M && valid) volume_scatter<DET, FAST>(sc, io, bw, s_df, si, tid, det, scr);
         }
         __syncthreads();
     }
+    if constexpr (STOP) stop_finish(smem, stop, tid);
 }
 
 // ---- fused Adam (torch.optim.Adam: no weight decay, no amsgrad) ---------------------------------------------
@@ -1021,11 +1210,12 @@ __device__ __forceinline__ int det_scale_exp(unsigned amax_bits, long long n) {
 
 // FAST (the rays entry): each sample's NDC is marched again from io.rays / io.t_steps / jitter by the function the
 // backward kernel's front end used (sample_point), so it has the same bits and needs no per-sample record.
-template <bool FAST>
+// STOP (FAST only): the samples j >= live[ray] are dead; their records were never written, so they are skipped.
+template <bool FAST, bool STOP = false>
 __global__ void det_scatter_kernel(const SceneDev sc, const float* __restrict__ ndc, const float* __restrict__ rec,
                                    const unsigned* __restrict__ amax, long long nsamp,
                                    unsigned long long* __restrict__ acc, float* __restrict__ dvol, const RenderIO io,
-                                   const float* __restrict__ jitter) {
+                                   const float* __restrict__ jitter, const int* __restrict__ live) {
     const unsigned mb = amax[0];
     if (mb == 0u && amax[1] == 0u) return;                      // all-zero gradients
     __shared__ Cams cams;
@@ -1039,6 +1229,10 @@ __global__ void det_scatter_kernel(const SceneDev sc, const float* __restrict__ 
     for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < nsamp * 64; t += (long long)gridDim.x * blockDim.x) {
         const long long si = t >> 6;
         const int c = (int)(t >> 3) & 7, ch = (int)t & 7;
+        if constexpr (STOP) {
+            const int ray = (int)(si / io.S);
+            if (si - (long long)ray * io.S >= __ldg(live + ray)) continue;
+        }
         const float g = __ldg(rec + si * 8 + ch);
         if (g == 0.f) continue;
         Trilinear tr;
@@ -1095,20 +1289,22 @@ static int bwd_grid(int N, int S) {
     return ngroups < sm_count() ? ngroups : sm_count();
 }
 
-// One backward-kernel launch of the variant (tc, DET, FAST); wh is the fp16 dgrad image (tc) or unused.
-template <bool DET, bool FAST>
+// One backward-kernel launch of the variant (tc, DET, FAST, STOP); wh is the fp16 dgrad image (tc) or unused.
+template <bool DET, bool FAST, bool STOP = false>
 static int launch_bwd_kernel(bool tc, int grid, const SceneDev& sc, const RenderIO& io, const BwdIO& bw, const float* wts,
-                             const __half* wh, const DetIO& dt, const float* jitter, cudaStream_t stream) {
+                             const __half* wh, const DetIO& dt, const float* jitter, cudaStream_t stream,
+                             const StopIO& stop = StopIO{}) {
     static bool attr_set[2][64] = {};
-    const void* kfn = tc ? (const void*)render_bwd_tc_kernel<DET, FAST> : (const void*)render_bwd_kernel<DET, FAST>;
+    const void* kfn = tc ? (const void*)render_bwd_tc_kernel<DET, FAST, STOP> : (const void*)render_bwd_kernel<DET, FAST, STOP>;
+    const size_t smem = BWD_SMEM_BYTES + (STOP ? STOP_SMEM_BYTES : 0);
     int dev = 0;
     MVSN_CUDA_CHECK(cudaGetDevice(&dev));
     if (dev >= 64 || !attr_set[tc][dev]) {
-        MVSN_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+        MVSN_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         if (dev < 64) attr_set[tc][dev] = true;
     }
-    if (tc) render_bwd_tc_kernel<DET, FAST><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts, wh, dt, jitter);
-    else    render_bwd_kernel<DET, FAST><<<grid, 256, BWD_SMEM_BYTES, stream>>>(sc, io, bw, wts, dt, jitter);
+    if (tc) render_bwd_tc_kernel<DET, FAST, STOP><<<grid, 256, smem, stream>>>(sc, io, bw, wts, wh, dt, jitter, stop);
+    else    render_bwd_kernel<DET, FAST, STOP><<<grid, 256, smem, stream>>>(sc, io, bw, wts, dt, jitter, stop);
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;
 }
@@ -1152,20 +1348,44 @@ size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, 
     return det_layout(base, N, S, (size_t)D * Hp * Wp).total;
 }
 
+// Early ray termination: the workspace of the grad mode and summation order, then (256-byte aligned) the [N] live
+// counts and the CTAs' deferred-ray lists, list_cap (ray, live samples) pairs per CTA: every ray of its phase-A groups.
+namespace {
+struct StopLayout { size_t live, list, total; int list_cap; };
+StopLayout stop_layout(size_t base, int N, int S) {
+    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const int R = TILE_M / S, ngroups = (N + R - 1) / R, grid = bwd_grid(N, S);
+    StopLayout l{};
+    l.list_cap = (ngroups + grid - 1) / grid * R;
+    l.live = up(base);
+    l.list = up(l.live + (size_t)N * sizeof(int));
+    l.total = l.list + (size_t)grid * l.list_cap * sizeof(int2);
+    return l;
+}
+}  // namespace
+
+size_t render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc, bool det) {
+    const size_t base = det ? render_backward_det_workspace_bytes(N, S, D, Hp, Wp, tc)
+                            : (tc ? render_backward_tc_workspace_bytes(N, S) : render_backward_workspace_bytes(N, S));
+    return base ? stop_layout(base, N, S).total : 0;
+}
+
 int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const float* const* mlp_w,
                            const float* g_rgb, const float* target, float inv_count, const float* g_depth,
                            const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
                            float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det, const float* jitter) {
+                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det, const float* jitter,
+                           const BwdStop* stop) {
     const bool fast = io.rays != nullptr;
-    const char* what = fast ? "mvsn_render_backward_rays"
+    const char* what = stop ? "mvsn_render_backward_rays_stop" : fast ? "mvsn_render_backward_rays"
                             : det ? (tc ? "deterministic render backward (grad_mode TC_HALF)" : "deterministic render backward")
                                   : (tc ? "render backward (grad_mode TC_HALF)" : "render backward");
     MVSN_REQUIRE(io.S <= TILE_M, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, io.S);
     const size_t base = tc ? render_backward_tc_workspace_bytes(io.N, io.S) : render_backward_workspace_bytes(io.N, io.S);
     const size_t nvox = dvol ? (size_t)sc.D * sc.Hp * sc.Wp : 0;
     const DetLayout dl = det_layout(base, io.N, io.S, nvox);
-    const size_t need = det ? dl.total : base;
+    const StopLayout sl = stop_layout(det ? dl.total : base, io.N, io.S);
+    const size_t need = stop ? sl.total : det ? dl.total : base;
     MVSN_REQUIRE(workspace && workspace_bytes >= need, MVSN_EWORKSPACE, "%s: workspace %zu < %zu bytes", what, workspace_bytes, need);
     MVSN_REQUIRE(aligned16(workspace), MVSN_EALIGN, "%s: workspace must be 16-byte aligned", what);
     DetIO dt{};
@@ -1197,7 +1417,18 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
         pack_dgrad_kernel<<<64, 256, 0, stream>>>(wp, wimg);
     }
     MVSN_CUDA_CHECK(cudaGetLastError());
-    const int rc = det ? (fast ? launch_bwd_kernel<true, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
+    StopIO st{};
+    if (stop) {
+        char* w8 = static_cast<char*>(workspace);
+        st.t_stop = stop->t_stop;
+        st.live = stop->live_samples ? stop->live_samples : reinterpret_cast<int*>(w8 + sl.live);
+        st.list = reinterpret_cast<int2*>(w8 + sl.list);
+        st.list_cap = sl.list_cap;
+        st.tiles_done = stop->tiles_done;
+    }
+    const int rc = stop ? (det ? launch_bwd_kernel<true, true, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st)
+                               : launch_bwd_kernel<false, true, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st))
+                 : det ? (fast ? launch_bwd_kernel<true, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
                                : launch_bwd_kernel<true, false>(tc, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream))
                        : (fast ? launch_bwd_kernel<false, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
                                : launch_bwd_kernel<false, false>(tc, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream));
@@ -1210,8 +1441,12 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
         const long long nsamp = (long long)io.N * io.S;
         auto* acc = reinterpret_cast<unsigned long long*>(static_cast<char*>(workspace) + dl.acc);
         const int gs = cdiv(nsamp * 64, 256) < sm_count() * 16 ? cdiv(nsamp * 64, 256) : sm_count() * 16;
-        if (fast) det_scatter_kernel<true><<<gs, 256, 0, stream>>>(sc, nullptr, dt.rec, dt.amax, nsamp, acc, dvol, io, jitter);
-        else      det_scatter_kernel<false><<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, dvol, io, nullptr);
+        if (stop) det_scatter_kernel<true, true><<<gs, 256, 0, stream>>>(sc, nullptr, dt.rec, dt.amax, nsamp, acc, dvol, io,
+                                                                         jitter, st.live);
+        else if (fast) det_scatter_kernel<true><<<gs, 256, 0, stream>>>(sc, nullptr, dt.rec, dt.amax, nsamp, acc, dvol, io,
+                                                                       jitter, nullptr);
+        else      det_scatter_kernel<false><<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, dvol, io, nullptr,
+                                                                   nullptr);
         MVSN_CUDA_CHECK(cudaGetLastError());
         const long long n2 = (long long)nvox * 4;               // (int64 pair, float pair) per thread step
         const int gc = cdiv(n2, 256) < sm_count() * 8 ? cdiv(n2, 256) : sm_count() * 8;

@@ -77,12 +77,15 @@ int pack_mlp_wg(const float* const* w, bool split, void* packed, cudaStream_t st
 size_t render_backward_workspace_bytes(int N, int S);
 size_t render_backward_tc_workspace_bytes(int N, int S);
 size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc);
+size_t render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc, bool det);
+// early ray termination of the rays backward (mvsn_render_backward_rays_stop); live_samples / tiles_done may be NULL
+struct BwdStop { float t_stop; int* live_samples; unsigned long long* tiles_done; };
 int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const float* const* mlp_w,
                            const float* g_rgb, const float* target, float inv_count, const float* g_depth,
                            const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
                            float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
                            size_t workspace_bytes, cudaStream_t stream, bool tc, bool det,
-                           const float* jitter = nullptr);
+                           const float* jitter = nullptr, const BwdStop* stop = nullptr);
 int launch_adam_tensors(float* const* p, const float* const* g, float* const* m, float* const* v, const int* n, int count,
                         float lr, float beta1, float beta2, float eps, int step, cudaStream_t stream);
 int launch_adam_volume(float* p, float* g_dhwc, float* m, float* v, long long nvox, int planar, float lr, float beta1,

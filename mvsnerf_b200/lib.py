@@ -33,6 +33,7 @@ EXPORTS = [
     "mvsn_render_backward_deterministic_workspace_bytes", "mvsn_render_backward_deterministic",
     "mvsn_render_backward_rays_workspace_bytes", "mvsn_render_backward_rays",
     "mvsn_render_rays_stop",
+    "mvsn_render_backward_rays_stop_workspace_bytes", "mvsn_render_backward_rays_stop",
 ]
 MAX_PEERS, PEER_HANDLE_BYTES = 16, 64
 BN_BATCH, BN_BATCH_UPDATE, BN_RUNNING = 0, 1, 2
@@ -118,6 +119,11 @@ def load() -> C.CDLL:
     lib.mvsn_render_backward_rays.argtypes = [C.POINTER(RenderScene), C.POINTER(vp), C.POINTER(RayParams), vp, vp, vp,
                                               ip, ip, ip, ip, C.POINTER(RenderGrads), C.POINTER(vp), vp, vp, C.c_size_t,
                                               vp]
+    lib.mvsn_render_backward_rays_stop_workspace_bytes.restype = C.c_size_t
+    lib.mvsn_render_backward_rays_stop_workspace_bytes.argtypes = [ip, ip, ip, ip, ip, ip, ip]
+    lib.mvsn_render_backward_rays_stop.argtypes = [C.POINTER(RenderScene), C.POINTER(vp), C.POINTER(RayParams), vp, vp,
+                                                   vp, ip, ip, ip, ip, fp, C.POINTER(RenderGrads), C.POINTER(vp), vp,
+                                                   vp, vp, vp, C.c_size_t, vp]
     lib.mvsn_adam_step.argtypes = [C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(ip), ip,
                                    fp, fp, fp, fp, ip, vp]
     lib.mvsn_adam_step_volume.argtypes = [vp, vp, vp, vp, C.c_longlong, ip, fp, fp, fp, fp, ip, vp]
@@ -131,7 +137,8 @@ def load() -> C.CDLL:
                  "mvsn_build_cost_volume", "mvsn_costreg_forward", "mvsn_featurenet_forward",
                  "mvsn_render_rays_to_peers", "mvsn_peer_buffer_create", "mvsn_peer_buffer_open",
                  "mvsn_peer_buffer_close", "mvsn_peer_buffer_destroy", "mvsn_render_backward", "mvsn_render_backward_tc",
-                 "mvsn_render_backward_deterministic", "mvsn_render_backward_rays", "mvsn_adam_step",
+                 "mvsn_render_backward_deterministic", "mvsn_render_backward_rays",
+                 "mvsn_render_backward_rays_stop", "mvsn_adam_step",
                  "mvsn_adam_step_volume", "mvsn_featurenet_forward_bn", "mvsn_costreg_forward_bn"):
         getattr(lib, name).restype = ip
     _lib = lib
