@@ -43,6 +43,12 @@ extern "C" {
 #define MVSN_MLP_TC_PAIR     3  /* same kernel and image as TC_HALF (the bench headline): weights     */
                                 /* streamed, activations in registers, views/feature layers folded  */
                                 /* (TC modes take any N_samples; rays are tiled up to 32 at a time)    */
+#define MVSN_VOLUME_F16      0x100 /* flag OR-ed into mvsn_render_scene.mlp_mode with a TC mode: volume_dhwc points at an */
+                                /* fp16 [D,Hp,Wp,8] image (16-byte aligned).  Each value is widened exactly to fp32, so a  */
+                                /* render is bit-identical to one from the fp32 volume vol.half().float(); the storage     */
+                                /* rounding is the only change.  Render entries only: with MVSN_MLP_FP32 and in every      */
+                                /* mvsn_render_backward* entry it gives MVSN_EUNSUPPORTED before any CUDA call;            */
+                                /* mvsn_mlp_pack / mvsn_mlp_packed_bytes ignore it.                                         */
 
 #define MVSN_N_MLP_TENSORS   22 /* network_fn_state_dict, reference models.py:145-222 / SURVEY App. B */
 #define MVSN_N_COSTREG_TENSORS 30 /* 10 x (conv weight, bn gamma, bn beta), models.py:725-769          */
@@ -79,6 +85,12 @@ int mvsn_volume_to_channels_last(const float* vol_cdhw, int D, int Hp, int Wp,
                                  float* vol_dhwc, void* stream);
 int mvsn_volume_from_channels_last(const float* vol_dhwc, int D, int Hp, int Wp,
                                    float* vol_cdhw, void* stream);
+/* fp16 volume image for MVSN_VOLUME_F16: src is planar [8,D,Hp,Wp] (src_planar != 0) or channels-last [D,Hp,Wp,8],
+ * fp32 or fp16 (src_half != 0), dense, aligned to its element size; vol_dhwc_f16 [D,Hp,Wp,8] fp16, 16-byte aligned.
+ * fp32 values are rounded with __float2half_rn, as Tensor.half() rounds them: beyond 65504 they become inf and fp16
+ * subnormals are kept.  Argument errors are returned before any CUDA call. */
+int mvsn_volume_to_half(const void* src, int src_half, int src_planar, int D, int Hp, int Wp, void* vol_dhwc_f16,
+                        void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Rendering  (replaces: renderer.rendering, renderer.py:138-165, and everything it calls:
@@ -88,14 +100,14 @@ int mvsn_volume_from_channels_last(const float* vol_dhwc, int D, int Hp, int Wp,
  *   raw2outputs/raw2alpha renderer.py:18-26,65-92)
  * ------------------------------------------------------------------------------------- */
 typedef struct mvsn_render_scene {
-    const float* volume_dhwc;   /* [D,Hp,Wp,8] channels-last encoding volume                    */
+    const float* volume_dhwc;   /* [D,Hp,Wp,8] channels-last encoding volume (fp16 with MVSN_VOLUME_F16) */
     int D, Hp, Wp;
     const float* imgs_hwc4;     /* [V,H,W,4] source images, from mvsn_pack_images               */
     int V, H, W;                /* V must be 3 (feat_dim = 8 + 4V = 20, train_mvs_nerf_pl.py:38) */
     const float* w2cs;          /* [V,4,4] device: world -> camera, pose_source['w2cs']           */
     const float* intrinsics;    /* [V,3,3] device: full-resolution K, pose_source['intrinsics']   */
     const void* mlp_packed;     /* from mvsn_mlp_pack                                             */
-    int mlp_mode;               /* MVSN_MLP_*                                                     */
+    int mlp_mode;               /* MVSN_MLP_*, optionally | MVSN_VOLUME_F16 (TC modes)            */
     int white_bkgd;             /* renderer.py:91-92                                              */
 } mvsn_render_scene;
 
@@ -357,6 +369,12 @@ int mvsn_featurenet_forward_bn(const float* const* w_host_array_of_device_ptrs, 
 int mvsn_costreg_forward_bn(const float* const* w_host_array_of_device_ptrs, float* const* running, int bn_mode,
                             float momentum, const float* cost, int D, int Hp, int Wp, float* volume_dhwc,
                             void* workspace, size_t workspace_bytes, void* stream);
+/* mvsn_costreg_forward_f16: mvsn_costreg_forward_bn with the volume written as fp16 [D,Hp,Wp,8] (16-byte aligned), each
+ * value the fp32 result rounded with __float2half_rn (bit-identical to .half() of mvsn_costreg_forward_bn's volume; the
+ * running statistics are updated identically): the input of MVSN_VOLUME_F16 renders without a conversion pass. */
+int mvsn_costreg_forward_f16(const float* const* w_host_array_of_device_ptrs, float* const* running, int bn_mode,
+                             float momentum, const float* cost, int D, int Hp, int Wp, void* volume_dhwc_f16,
+                             void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Diagnostic: one 128 x N x K fp16 GEMM (fp32 accumulate) through the same wgmma building blocks

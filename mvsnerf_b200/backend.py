@@ -169,21 +169,25 @@ class CostRegNet(nn.Module):
             out.append(m.bn if isinstance(m, ConvBnReLU3D) else m[1])
         return out
 
-    def forward(self, cost):
+    def forward(self, cost, volume_dtype=torch.float32):
         """cost [1,41,D,Hp,Wp] (reference layout) -> [1,8,D,Hp,Wp] (channels-last memory).  BatchNorm dispatches on
-        `self.training` (models.py:674-685): batch statistics (+ running update) in train mode, running in eval."""
+        `self.training` (models.py:674-685): batch statistics (+ running update) in train mode, running in eval.
+        volume_dtype=torch.float16: the volume is stored as fp16, bit-identical to .half() of the fp32 volume."""
+        if volume_dtype not in (torch.float32, torch.float16):
+            raise RuntimeError(f"CostRegNet: volume_dtype {volume_dtype} (torch.float32 or torch.float16)")
         lib = _lib.load()
         cost = _lib.dev_f32(cost, "cost volume")
         _, _, D, Hp, Wp = cost.shape
         ws_bytes = lib.mvsn_costreg_workspace_bytes(D, Hp, Wp)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=cost.device)
-        vol = torch.empty(D, Hp, Wp, 8, dtype=torch.float32, device=cost.device)
+        vol = torch.empty(D, Hp, Wp, 8, dtype=volume_dtype, device=cost.device)
         weights = [_lib.dev_f32(w.detach(), "CostRegNet weight") for w in self.weight_list()]
         running, mode, momentum = _bn_call_args(self.bn_modules(), self.training)
+        entry = "mvsn_costreg_forward_bn" if volume_dtype == torch.float32 else "mvsn_costreg_forward_f16"
         with torch.cuda.device(cost.device):
-            _lib.check(lib.mvsn_costreg_forward_bn(_lib.ptr_array(weights), _lib.ptr_array(running), mode, momentum,
-                                                   _lib.ptr(cost), D, Hp, Wp, _lib.ptr(vol), _lib.ptr(ws), ws_bytes,
-                                                   _lib.stream_ptr()), "mvsn_costreg_forward_bn")
+            _lib.check(getattr(lib, entry)(_lib.ptr_array(weights), _lib.ptr_array(running), mode, momentum,
+                                           _lib.ptr(cost), D, Hp, Wp, _lib.ptr(vol), _lib.ptr(ws), ws_bytes,
+                                           _lib.stream_ptr()), entry)
         return vol.permute(3, 0, 1, 2).unsqueeze(0)
 
 
@@ -229,7 +233,9 @@ class MVSNet(nn.Module):
                        "mvsn_build_cost_volume")
         return cost, masks
 
-    def forward(self, imgs, proj_mats, near_far, pad=0, return_color=False, lindisp=False):
+    def forward(self, imgs, proj_mats, near_far, pad=0, return_color=False, lindisp=False, volume_dtype=torch.float32):
+        """volume_dtype=torch.float16: the encoding volume is returned in fp16 (channels-last, half the bytes),
+        bit-identical to .half() of the fp32 volume; the tensor-core render modes read it as it is."""
         if not imgs.is_cuda:
             raise RuntimeError("MVSNet: inputs must be CUDA tensors; mvsnerf_b200 has no CPU path")
         if torch.is_grad_enabled() and (imgs.requires_grad or any(p.requires_grad for p in self.parameters())):
@@ -251,7 +257,7 @@ class MVSNet(nn.Module):
         cost, in_masks = self.build_volume_costvar_img(imgs, feats_l, proj_mats, depth_values, pad=pad)
         if return_color:
             feats_l = torch.cat((cost[:, :V * 3].view(B, V, 3, *cost.shape[2:]), in_masks.unsqueeze(2)), dim=2)
-        volume = self.cost_reg_2(cost)
+        volume = self.cost_reg_2(cost, volume_dtype)
         return volume, feats_l, depth_values
 
 
@@ -386,8 +392,9 @@ def clear_cache():
     _cache.clear()
 
 
-def _volume_channels_last(volume_feature):
-    """Accepts a tensor [1,8,D,Hp,Wp] (any strides) or a RefVolume; returns ([D,Hp,Wp,8] fp32, dims)."""
+def _volume_channels_last(volume_feature, half_ok=False):
+    """Accepts a tensor [1,8,D,Hp,Wp] (any strides) or a RefVolume; returns ([D,Hp,Wp,8] fp32, dims).  With `half_ok`
+    (a tensor-core render), a float16 volume is returned as an fp16 image instead (MVSN_VOLUME_F16)."""
     owner = volume_feature.feat_volume if isinstance(volume_feature, nn.Module) else volume_feature
     vol = owner.detach()          # a NEW tensor object every call: the cache below is keyed on `owner`
     if vol.dim() != 5 or vol.shape[0] != 1 or vol.shape[1] != 8:
@@ -396,6 +403,20 @@ def _volume_channels_last(volume_feature):
         raise RuntimeError("encoding volume must be a CUDA tensor; mvsnerf_b200 has no CPU path")
     _, _, D, Hp, Wp = vol.shape
     cl = vol[0].permute(1, 2, 3, 0)
+    if half_ok and vol.dtype == torch.float16:
+        if cl.is_contiguous():
+            return cl, (D, Hp, Wp)                     # MVSNet.forward(volume_dtype=float16) or .half() of it: zero-copy
+
+        def build_f16():
+            lib = _lib.load()
+            src = vol[0].contiguous()                  # planar [8,D,Hp,Wp]: a view for a contiguous volume
+            dst = torch.empty(D, Hp, Wp, 8, dtype=torch.float16, device=vol.device)
+            with torch.cuda.device(vol.device):
+                _lib.check(lib.mvsn_volume_to_half(_lib.ptr(src), 1, 1, D, Hp, Wp, _lib.ptr(dst), _lib.stream_ptr()),
+                           "mvsn_volume_to_half")
+            return dst
+
+        return _cached("volume_f16", owner, build_f16), (D, Hp, Wp)
     if vol.dtype == torch.float32 and cl.is_contiguous():
         return cl, (D, Hp, Wp)                         # MVSNet.forward output: zero-copy
 
@@ -431,8 +452,10 @@ def _images_packed(imgs):
     return _cached("imgs", imgs, build), (V, H, W)
 
 
-def _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode):
-    vol, (D, Hp, Wp) = _volume_channels_last(volume_feature)
+def _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode, half_ok=False):
+    """half_ok: a forward render that may read a float16 volume as fp16 (tensor-core modes only); otherwise a half
+    volume is upcast to a cached fp32 image."""
+    vol, (D, Hp, Wp) = _volume_channels_last(volume_feature, half_ok and mode != _lib.MLP_FP32)
     im, (V, H, W) = _images_packed(imgs)
     if V != 3:
         raise RuntimeError(f"{V} source views: the v0 network takes exactly 3 (feat_dim = 8 + 3*4)")
@@ -446,6 +469,8 @@ def _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode):
                            f"{tuple(w2cs.shape)} and {tuple(intr.shape)}")
     sc.w2cs, sc.intrinsics = w2cs.data_ptr(), intr.data_ptr()
     packed = network_fn.packed(mode)
+    if vol.dtype == torch.float16:
+        mode |= _lib.VOLUME_F16
     sc.mlp_packed, sc.mlp_mode, sc.white_bkgd = packed.data_ptr(), mode, int(bool(white_bkgd))
     keep = (vol, im, packed, w2cs, intr)          # keep the device buffers alive for the duration of the call
     return sc, keep
@@ -487,13 +512,14 @@ def rendering(args, pose_ref, rays_pts, rays_ndc, depth_candidates, rays_o, rays
             bool(white_bkgd), mode, network_fn, volume_feature, grad_mode, *params)
         return rgb, feat, weights, depth, alpha, {}
     rgb, feat, weights, depth, alpha = _render_samples_kernel(
-        pose_ref, rays_pts, rays_ndc, z, rays_dir, volume_feature, imgs, network_fn, white_bkgd, mode, want_aux)
+        pose_ref, rays_pts, rays_ndc, z, rays_dir, volume_feature, imgs, network_fn, white_bkgd, mode, want_aux,
+        half_ok=True)
     return rgb, feat, weights, depth, alpha, {}
 
 
 def _render_samples_kernel(pose_ref, rays_pts, rays_ndc, z, rays_dir, volume_feature, imgs, network_fn, white_bkgd,
-                           mode, want_aux=True):
-    """One mvsn_render_samples launch (no autograd graph)."""
+                           mode, want_aux=True, half_ok=False):
+    """One mvsn_render_samples launch (no autograd graph); half_ok: see _make_scene."""
     lib = _lib.load()
     N, S = rays_pts.shape[:2]
     dev = rays_pts.device
@@ -501,7 +527,7 @@ def _render_samples_kernel(pose_ref, rays_pts, rays_ndc, z, rays_dir, volume_fea
     ndc = _lib.dev_f32(rays_ndc.detach(), "rays_ndc")
     z = _lib.dev_f32(z.detach(), "depth_candidates")
     dirs = _lib.dev_f32(rays_dir.detach(), "rays_dir")
-    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode)
+    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode, half_ok)
     rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
     depth = torch.empty(N, dtype=torch.float32, device=dev)
     feat = weights = alpha = None
@@ -1034,7 +1060,11 @@ def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
     `t_stop` (a float >= 0, tensor-core modes): early ray termination (mvsn_render_rays_stop) -- a group of up to 32
     neighbouring rays stops two tiles (four samples at frame sizes) after every ray in it has transmittance < t_stop, so
     each channel differs from the full render by less than t_stop (t_stop = 0: bit-identical).  `tiles_done`: an
-    optional CUDA int64 tensor [1] the number of computed 64-sample tiles is added to.  Not combinable with `sink`."""
+    optional CUDA int64 tensor [1] the number of computed 64-sample tiles is added to.  Not combinable with `sink`.
+
+    A float16 `volume_feature` is read as fp16 in the tensor-core modes (half the resident bytes): the result is
+    bit-identical to rendering `volume.float()`.  Channels-last storage (MVSNet.forward(..., volume_dtype=torch.float16),
+    or `.half()` of an fp32 MVSNet volume) is read in place; other layouts are converted once per tensor version."""
     lib = _lib.load()
     mode = DEFAULT_MLP_MODE if mlp_mode is None else mlp_mode
     if t_stop is not None:
@@ -1053,7 +1083,7 @@ def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
     dev = rays.device
     S = int(N_samples)
     t_steps = _tsteps_of(S, dev)
-    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode)
+    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode, half_ok=True)
     rp = _lib.RayParams(float(near_far[0]), float(near_far[1]), float(pad), int(bool(lindisp)))
     if out is not None:
         rgb, depth = out

@@ -134,16 +134,22 @@ static int make_scene(const mvsn_render_scene* s, SceneDev& d) {
     return MVSN_OK;
 }
 
+// scene->mlp_mode without / with the MVSN_VOLUME_F16 flag
+static int mlp_mode_of(const mvsn_render_scene* scene) { return scene->mlp_mode & ~MVSN_VOLUME_F16; }
+static bool half_volume(const mvsn_render_scene* scene) { return (scene->mlp_mode & MVSN_VOLUME_F16) != 0; }
+
 static int dispatch_render(const mvsn_render_scene* scene, const SceneDev& sc, const RenderIO& io, bool fast,
                            cudaStream_t stream) {
-    switch (scene->mlp_mode) {
+    const bool hv = half_volume(scene);
+    switch (mlp_mode_of(scene)) {
         case MVSN_MLP_FP32:
+            MVSN_REQUIRE(!hv, MVSN_EUNSUPPORTED, "MVSN_MLP_FP32 reads an fp32 volume only (MVSN_VOLUME_F16 given)");
             return launch_render_fp32(sc, io, fast, static_cast<const float*>(scene->mlp_packed), stream);
         case MVSN_MLP_TC_HALF:
         case MVSN_MLP_TC_PAIR:
-            return launch_render_wg(sc, io, fast, false, scene->mlp_packed, stream);
+            return launch_render_wg(sc, io, fast, false, scene->mlp_packed, stream, nullptr, nullptr, hv);
         case MVSN_MLP_TC_SPLIT:
-            return launch_render_wg(sc, io, fast, true, scene->mlp_packed, stream);
+            return launch_render_wg(sc, io, fast, true, scene->mlp_packed, stream, nullptr, nullptr, hv);
         default:
             set_error("mlp_mode %d is not available in this build", scene->mlp_mode);
             return MVSN_EUNSUPPORTED;
@@ -160,7 +166,7 @@ const char* mvsn_last_error(void) { return g_err; }
 int mvsn_abi_version(void) { return 2; }
 
 size_t mvsn_mlp_packed_bytes(int mode) {
-    switch (mode) {
+    switch (mode & ~MVSN_VOLUME_F16) {
         case MVSN_MLP_FP32: return (size_t)w32::TOTAL * sizeof(float);
         case MVSN_MLP_TC_HALF:
         case MVSN_MLP_TC_PAIR: return mlp_wg_packed_bytes(false);
@@ -171,6 +177,7 @@ size_t mvsn_mlp_packed_bytes(int mode) {
 
 int mvsn_mlp_pack(const float* const* w, int mode, void* packed, size_t packed_bytes, void* stream) {
     MVSN_RANGE("mvsn_mlp_pack");
+    mode &= ~MVSN_VOLUME_F16;                             // the weight image does not depend on the volume's storage
     MVSN_REQUIRE(w && packed, MVSN_ENULL, "mvsn_mlp_pack: NULL argument");
     const size_t need = mvsn_mlp_packed_bytes(mode);
     MVSN_REQUIRE(need != 0, MVSN_EUNSUPPORTED, "mvsn_mlp_pack: mode %d not available", mode);
@@ -219,6 +226,18 @@ int mvsn_volume_from_channels_last(const float* src, int D, int Hp, int Wp, floa
         reinterpret_cast<const float4*>(src), dst, n);
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;
+}
+
+int mvsn_volume_to_half(const void* src, int src_half, int src_planar, int D, int Hp, int Wp, void* vol_dhwc_f16,
+                        void* stream) {
+    MVSN_RANGE("mvsn_volume_to_half");
+    MVSN_REQUIRE(src && vol_dhwc_f16, MVSN_ENULL, "mvsn_volume_to_half: NULL argument");
+    MVSN_REQUIRE(D > 0 && Hp > 0 && Wp > 0, MVSN_EBADSHAPE, "mvsn_volume_to_half: D=%d Hp=%d Wp=%d", D, Hp, Wp);
+    MVSN_REQUIRE(aligned16(vol_dhwc_f16), MVSN_EALIGN, "mvsn_volume_to_half: output must be 16-byte aligned");
+    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(src) % (src_half ? 2 : 4) == 0, MVSN_EALIGN,
+                 "mvsn_volume_to_half: input not aligned to its element size");
+    const long long n = (long long)D * Hp * Wp;
+    return launch_volume_to_half(src, src_half != 0, src_planar != 0, n, vol_dhwc_f16, (cudaStream_t)stream);
 }
 
 int mvsn_render_samples(const mvsn_render_scene* scene, const float* rays_pts, const float* rays_ndc,
@@ -304,8 +323,8 @@ int mvsn_render_rays_stop(const mvsn_render_scene* scene, const mvsn_ray_params*
     MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "mvsn_render_rays_stop: N=%d S=%d", N, S);
     MVSN_REQUIRE(rays && t_steps && rgb && depth, MVSN_ENULL, "mvsn_render_rays_stop: NULL required pointer");
     MVSN_REQUIRE(t_stop >= 0.f, MVSN_EBADSHAPE, "mvsn_render_rays_stop: t_stop=%g must be >= 0 (not NaN)", (double)t_stop);
-    MVSN_REQUIRE(scene->mlp_mode == MVSN_MLP_TC_HALF || scene->mlp_mode == MVSN_MLP_TC_PAIR ||
-                     scene->mlp_mode == MVSN_MLP_TC_SPLIT,
+    const int mode = mlp_mode_of(scene);
+    MVSN_REQUIRE(mode == MVSN_MLP_TC_HALF || mode == MVSN_MLP_TC_PAIR || mode == MVSN_MLP_TC_SPLIT,
                  MVSN_EUNSUPPORTED, "mvsn_render_rays_stop: mlp_mode %d has no early ray termination (tensor-core modes only)",
                  scene->mlp_mode);
     MVSN_REQUIRE(aligned16(rays), MVSN_EALIGN, "rays must be 16-byte aligned");
@@ -317,8 +336,8 @@ int mvsn_render_rays_stop(const mvsn_render_scene* scene, const mvsn_ray_params*
     io.N = N; io.S = S;
     io.rgb = rgb; io.depth = depth;
     io.rg = make_ray_gen(scene, rp);
-    return launch_render_wg(sc, io, true, scene->mlp_mode == MVSN_MLP_TC_SPLIT, scene->mlp_packed, (cudaStream_t)stream,
-                            &t_stop, tiles_done);
+    return launch_render_wg(sc, io, true, mode == MVSN_MLP_TC_SPLIT, scene->mlp_packed, (cudaStream_t)stream,
+                            &t_stop, tiles_done, half_volume(scene));
 }
 
 int mvsn_render_rays_to_peers(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const float* rays,

@@ -12,6 +12,7 @@
 // channels; a warp owns 32 consecutive strips, so input rows are fetched with one 16-byte load per
 // lane and the +-1 halo comes from the neighbouring lanes by shuffle.  Weights for the CTA's CT
 // output channels sit in shared memory ([cin][27][CT], read as broadcast LDS.128).
+#include <cuda_fp16.h>
 #include "conv_common.cuh"
 
 namespace mvsn {
@@ -454,7 +455,9 @@ deconv3d_subpixel_kernel(const ConvArgs a) {
 
 // ------------------------------------------------------------------------------------------
 // final: volume = ABN(conv0) + ABN(deconv11)  -> channels-last [nvox][8]   (models.py:766)
+// F16: the fp32 sums rounded with __float2half_rn, one 16-byte store of eight halves per voxel
 // ------------------------------------------------------------------------------------------
+template <bool F16>
 __global__ void __launch_bounds__(256)
 finalize_volume_kernel(ActSrc s0, ActSrc s1, long long nvox, float4* __restrict__ out) {
     __shared__ float sc[2][8], sh[2][8];
@@ -466,8 +469,17 @@ finalize_volume_kernel(ActSrc s0, ActSrc s1, long long nvox, float4* __restrict_
 #pragma unroll
         for (int c = 0; c < 8; ++c)
             v[c] = act(__ldg(s0.x + c * nvox + i), sc[0][c], sh[0][c]) + act(__ldg(s1.x + c * nvox + i), sc[1][c], sh[1][c]);
-        out[2 * i] = make_float4(v[0], v[1], v[2], v[3]);
-        out[2 * i + 1] = make_float4(v[4], v[5], v[6], v[7]);
+        if constexpr (F16) {
+            uint32_t h[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                h[j] = (uint32_t)__half_as_ushort(__float2half_rn(v[2 * j])) |
+                       ((uint32_t)__half_as_ushort(__float2half_rn(v[2 * j + 1])) << 16);
+            reinterpret_cast<uint4*>(out)[i] = make_uint4(h[0], h[1], h[2], h[3]);
+        } else {
+            out[2 * i] = make_float4(v[0], v[1], v[2], v[3]);
+            out[2 * i + 1] = make_float4(v[4], v[5], v[6], v[7]);
+        }
     }
 }
 
@@ -544,6 +556,10 @@ static const int kLevelOut[10] = {0, 1, 1, 2, 2, 3, 3, 2, 1, 0};     // resoluti
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+static int costreg_forward(const float* const* w, float* const* running, int bn_mode, float momentum, const float* cost,
+                           int D, int Hp, int Wp, void* volume_dhwc, bool f16, void* workspace, size_t workspace_bytes,
+                           void* stream_);
+
 extern "C" {
 
 size_t mvsn_costreg_workspace_bytes(int D, int Hp, int Wp) {
@@ -565,6 +581,24 @@ int mvsn_costreg_forward(const float* const* w, const float* cost, int D, int Hp
 int mvsn_costreg_forward_bn(const float* const* w, float* const* running, int bn_mode, float momentum, const float* cost,
                             int D, int Hp, int Wp, float* volume_dhwc, void* workspace, size_t workspace_bytes, void* stream_) {
     MVSN_RANGE("mvsn_costreg_forward_bn");
+    return costreg_forward(w, running, bn_mode, momentum, cost, D, Hp, Wp, volume_dhwc, false, workspace, workspace_bytes,
+                           stream_);
+}
+
+int mvsn_costreg_forward_f16(const float* const* w, float* const* running, int bn_mode, float momentum, const float* cost,
+                             int D, int Hp, int Wp, void* volume_dhwc_f16, void* workspace, size_t workspace_bytes,
+                             void* stream_) {
+    MVSN_RANGE("mvsn_costreg_forward_f16");
+    return costreg_forward(w, running, bn_mode, momentum, cost, D, Hp, Wp, volume_dhwc_f16, true, workspace,
+                           workspace_bytes, stream_);
+}
+
+}  // extern "C"
+
+// mvsn_costreg_forward_bn (f16 = false: fp32 volume) and mvsn_costreg_forward_f16
+static int costreg_forward(const float* const* w, float* const* running, int bn_mode, float momentum, const float* cost,
+                           int D, int Hp, int Wp, void* volume_dhwc, bool f16, void* workspace, size_t workspace_bytes,
+                           void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     const bool conv0_ffma_flag = (bn_mode & MVSN_CONV0_FFMA) != 0;
     bn_mode &= ~MVSN_CONV0_FFMA;
@@ -636,8 +670,9 @@ int mvsn_costreg_forward_bn(const float* const* w, float* const* running, int bn
     if ((rc = launch_deconv(args(8, src(4), src(7), dims[7]), st))) return rc;             // conv9  (conv4 + .) 32->16
     if ((rc = launch_deconv(args(9, src(2), src(8), dims[8]), st))) return rc;              // conv11 (conv2 + .) 16->8
     const long long nvox = full.n();
-    finalize_volume_kernel<<<cdiv(nvox, 256) < sm_count() * 8 ? cdiv(nvox, 256) : sm_count() * 8, 256, 0, st>>>(
-        src(0), src(9), nvox, reinterpret_cast<float4*>(volume_dhwc));
+    const int fgrid = cdiv(nvox, 256) < sm_count() * 8 ? cdiv(nvox, 256) : sm_count() * 8;
+    if (f16) finalize_volume_kernel<true><<<fgrid, 256, 0, st>>>(src(0), src(9), nvox, reinterpret_cast<float4*>(volume_dhwc));
+    else     finalize_volume_kernel<false><<<fgrid, 256, 0, st>>>(src(0), src(9), nvox, reinterpret_cast<float4*>(volume_dhwc));
     MVSN_CUDA_CHECK(cudaGetLastError());
     if (bn_mode == MVSN_BN_BATCH_UPDATE) {
         BnUpdateArgs u{};
@@ -651,5 +686,3 @@ int mvsn_costreg_forward_bn(const float* const* w, float* const* running, int bn
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;
 }
-
-}  // extern "C"

@@ -2,12 +2,14 @@
 // "a ray" and "the 86-channel MLP input" (renderer.py:138-165 and callees), as device functions
 // shared by the fp32 and the tensor-core (wgmma) render kernels.
 #pragma once
+#include <cuda_fp16.h>
+#include <type_traits>
 #include "common.cuh"
 
 namespace mvsn {
 
 struct SceneDev {
-    const float* vol;      // [D,Hp,Wp,8]
+    const float* vol;      // [D,Hp,Wp,8]; fp16 halves (read as such) in the half-volume render instantiations
     const float4* imgs;    // [V,H,W] texels (r,g,b,0)
     int D, Hp, Wp;
     int V, H, W;
@@ -65,9 +67,12 @@ __device__ __forceinline__ void store_pixel(const RenderIO& io, int ray, float r
 
 int launch_render_fp32(const SceneDev& sc, const RenderIO& io, bool fast, const float* wts, cudaStream_t stream);
 // tensor-core modes (render_wg.cu): split = MVSN_MLP_TC_SPLIT, otherwise the fp16-operand modes.  t_stop != NULL
-// (fast only): early ray termination at transmittance *t_stop; tiles_done (may be NULL) += the tiles computed
+// (fast only): early ray termination at transmittance *t_stop; tiles_done (may be NULL) += the tiles computed.
+// half_vol: sc.vol is an fp16 [D,Hp,Wp,8] image (MVSN_VOLUME_F16)
 int launch_render_wg(const SceneDev& sc, const RenderIO& io, bool fast, bool split, const void* wimg, cudaStream_t stream,
-                     const float* t_stop = nullptr, unsigned long long* tiles_done = nullptr);
+                     const float* t_stop = nullptr, unsigned long long* tiles_done = nullptr, bool half_vol = false);
+// fp16 [D,Hp,Wp,8] image of a planar [8,D,Hp,Wp] or channels-last volume, fp32 or fp16, rounded with __float2half_rn
+int launch_volume_to_half(const void* src, bool src_half, bool src_planar, long long nvox, void* dst, cudaStream_t stream);
 size_t mlp_wg_packed_bytes(bool split);
 int pack_mlp_wg(const float* const* w, bool split, void* packed, cudaStream_t stream);
 // fine-tuning step (render_bwd.cu); tc: dgrad / wgrad GEMMs on wgmma with fp16 operands (grad_mode TC_HALF);
@@ -205,6 +210,10 @@ __device__ __forceinline__ Trilinear trilinear_corners(const SceneDev& sc, float
 // utils.index_point_feature (utils.py:357-383): trilinear, zeros padding, align_corners=True.
 // All sixteen 16-byte loads are issued unconditionally (indices clamped, out-of-volume corners get
 // weight 0) so they are in flight together instead of one DRAM latency per corner.
+// VT = __half: sc.vol points at an fp16 [D,Hp,Wp,8] image, one 16-byte load per corner (eight in flight); every value
+// is widened exactly (__half2float) and enters the same FMAs in the same order, so the result is bit-identical to the
+// fp32 path on the volume `vol.half().float()`.
+template <typename VT = float>
 __device__ __forceinline__ void sample_volume(const SceneDev& sc, float nx, float ny, float nz, float* out8) {
     const int W = sc.Wp, H = sc.Hp, D = sc.D;
     Trilinear t = trilinear_corners(sc, nx, ny, nz);
@@ -218,11 +227,26 @@ __device__ __forceinline__ void sample_volume(const SceneDev& sc, float nx, floa
         xo[d] = min(max(x, 0), W - 1); yo[d] = min(max(y, 0), H - 1); zo[d] = min(max(z, 0), D - 1);
     }
     float4 va[8], vb[8];
+    if constexpr (std::is_same<VT, __half>::value) {
+        uint4 hv[8];
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        const float4* p = reinterpret_cast<const float4*>(
-            sc.vol + (((size_t)zo[c >> 2] * H + yo[(c >> 1) & 1]) * W + xo[c & 1]) * 8);
-        va[c] = __ldg(p); vb[c] = __ldg(p + 1);
+        for (int c = 0; c < 8; ++c)
+            hv[c] = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(sc.vol) +
+                                                         (((size_t)zo[c >> 2] * H + yo[(c >> 1) & 1]) * W + xo[c & 1]) * 8));
+        auto lo = [](uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u & 0xffffu))); };
+        auto hi = [](uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u >> 16))); };
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            va[c] = make_float4(lo(hv[c].x), hi(hv[c].x), lo(hv[c].y), hi(hv[c].y));
+            vb[c] = make_float4(lo(hv[c].z), hi(hv[c].z), lo(hv[c].w), hi(hv[c].w));
+        }
+    } else {
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const float4* p = reinterpret_cast<const float4*>(
+                sc.vol + (((size_t)zo[c >> 2] * H + yo[(c >> 1) & 1]) * W + xo[c & 1]) * 8);
+            va[c] = __ldg(p); vb[c] = __ldg(p + 1);
+        }
     }
 #pragma unroll
     for (int c = 0; c < 8; ++c) out8[c] = 0.f;

@@ -276,7 +276,8 @@ __device__ __forceinline__ void store_pe_cos(uint8_t* pe, int row, const float* 
     for (int c = 0; c < 4; ++c) store8<SPLIT>(pe, row, 4 + c, v + 8 * c);
 }
 // MISC cols 0..7 (volume), 24..31 (zero), 32..39 (view direction), 40..47 (zero); input_feat[0..7]
-template <bool SPLIT>
+// VT: the volume's storage type (float, or __half for an fp16 volume)
+template <bool SPLIT, typename VT>
 __device__ __forceinline__ void store_volume_dir(const SceneDev& sc, const Cams& cams, const RenderIO& io, const TileRow& r,
                                                  const float* nd, float dx, float dy, float dz, uint8_t* misc, int row) {
     float feat[8], dir[3] = {0.f, 0.f, 0.f};
@@ -284,7 +285,7 @@ __device__ __forceinline__ void store_volume_dir(const SceneDev& sc, const Cams&
     for (int i = 0; i < 8; ++i) feat[i] = 0.f;
     if (r.valid) {
         view_dir<SPLIT>(cams, dx, dy, dz, dir);
-        sample_volume(sc, nd[0], nd[1], nd[2], feat);
+        sample_volume<VT>(sc, nd[0], nd[1], nd[2], feat);
         if (io.input_feat) {
             float4* o = reinterpret_cast<float4*>(io.input_feat + r.si * 20);
             o[0] = make_float4(feat[0], feat[1], feat[2], feat[3]);
@@ -317,7 +318,7 @@ __device__ __forceinline__ void store_color(const SceneDev& sc, const Cams& cams
     store8<SPLIT>(misc, row, 1, feat);
     store8<SPLIT>(misc, row, 2, feat + 8);
 }
-template <bool FAST, bool SPLIT>
+template <bool FAST, bool SPLIT, typename VT>
 __device__ __forceinline__ void front_end(const SceneDev& sc, const Cams& cams, const RenderIO& io, int grp, int tile,
                                           int t, uint8_t* pe, uint8_t* misc) {
     const int row = t & (wg::ROWS - 1), part = t >> 6;
@@ -327,10 +328,10 @@ __device__ __forceinline__ void front_end(const SceneDev& sc, const Cams& cams, 
     if (r.valid) sample_point<FAST, SPLIT>(sc, cams, io, r.ray, r.s_idx, r.si, px, py, pz, dx, dy, dz, nx, ny, nz, z);
     const float nd[3] = {nx, ny, nz};
     if (part == 0) {
-        if (!SPLIT) store_volume_dir<SPLIT>(sc, cams, io, r, nd, dx, dy, dz, misc, row);
+        if (!SPLIT) store_volume_dir<SPLIT, VT>(sc, cams, io, r, nd, dx, dy, dz, misc, row);
         store_pe_sin<SPLIT>(pe, row, nd);
     } else {
-        if (SPLIT) store_volume_dir<SPLIT>(sc, cams, io, r, nd, dx, dy, dz, misc, row);
+        if (SPLIT) store_volume_dir<SPLIT, VT>(sc, cams, io, r, nd, dx, dy, dz, misc, row);
         store_color<SPLIT>(sc, cams, io, r, px, py, pz, misc, row);
         store_pe_cos<SPLIT>(pe, row, nd);
     }
@@ -348,7 +349,8 @@ template <> struct StopRegs<false> { static constexpr bool last = false; };
 // demand), or idle.  Tile k + 2 depends only on the verdicts up to tile k - 1, so every plan is known two passes ahead
 // and the producer fills a slot as soon as its consumer releases it, as without STOP.  Without STOP the kernel is the
 // one it always was (t_stop and tiles_done are unused).
-template <bool FAST, bool SPLIT, bool STOP = false>
+// VT = __half: the encoding volume is stored as fp16 (sc.vol points at halves); only the volume gather changes.
+template <bool FAST, bool SPLIT, bool STOP = false, typename VT = float>
 __global__ void __launch_bounds__(wg::threads(SPLIT), 1)
 render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict__ wimg, float t_stop,
                  unsigned long long* tiles_done) {
@@ -453,7 +455,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                     const int s = 2 * w + (filled[w] & 1);
                     if (filled[w] >= 2) mbar_wait(&sh.slot_empty[s], ((filled[w] >> 1) - 1) & 1);
                     uint8_t* pe = smem + s * SLOT_BYTES;
-                    front_end<FAST, false>(sc, sh.cams, io, grp, STOP ? pl[w].y : pass % NT, t, pe, pe + tile_bytes(false));
+                    front_end<FAST, false, VT>(sc, sh.cams, io, grp, STOP ? pl[w].y : pass % NT, t, pe, pe + tile_bytes(false));
                     fence_proxy_async();
                     mbar_arrive(&sh.slot_full[s]);
                     ++filled[w];
@@ -544,7 +546,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             // -------------------------- front end (split mode: this warpgroup's own operand tiles) -------------
             uint8_t* pe = smem + wgi * wg_bytes(true);
             uint8_t* misc = pe + off_misc(true);
-            front_end<FAST, true>(sc, sh.cams, io, grp, tile, t, pe, misc);
+            front_end<FAST, true, VT>(sc, sh.cams, io, grp, tile, t, pe, misc);
             fence_proxy_async();
             named_bar_sync(1 + wgi, 128);
             pe_u = smem_u32(pe); misc_u = smem_u32(misc);
@@ -733,22 +735,48 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
     }
 }
 
+// the dynamic shared memory of the six instantiations with volume storage VT
+template <typename VT>
+static int set_wg_smem_attributes() {
+    using namespace wg;
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false)));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, false, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false)));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, true, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false, true, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         smem_bytes(false) + STOP_BYTES));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, true, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         smem_bytes(true) + STOP_BYTES));
+    return MVSN_OK;
+}
+
+template <typename VT>
+static void launch_wg_kernel(int grid, int nthreads, int smem, cudaStream_t stream, const SceneDev& sc, const RenderIO& io,
+                             const uint8_t* w, bool fast, bool split, const float* t_stop, unsigned long long* tiles_done) {
+    using namespace wg;
+    if (t_stop) {                                         // early ray termination: the ray entry only
+        if (split) render_wg_kernel<true, true, true, VT><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done);
+        else       render_wg_kernel<true, false, true, VT><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done);
+    } else if (split) {
+        if (fast) render_wg_kernel<true, true, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
+        else      render_wg_kernel<false, true, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
+    } else {
+        if (fast) render_wg_kernel<true, false, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
+        else      render_wg_kernel<false, false, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
+    }
+}
+
 int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool split, const void* wimg, cudaStream_t stream,
-                     const float* t_stop, unsigned long long* tiles_done) {
+                     const float* t_stop, unsigned long long* tiles_done, bool half_vol) {
     using namespace wg;
     RenderIO io = io_in;
     static bool attr_set[64] = {false};                   // once per device, not per launch
     int dev = 0;
     MVSN_CUDA_CHECK(cudaGetDevice(&dev));
     if (dev >= 64 || !attr_set[dev]) {
-        MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false)));
-        MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false)));
-        MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
-        MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
-        MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             smem_bytes(false) + STOP_BYTES));
-        MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             smem_bytes(true) + STOP_BYTES));
+        int rc = set_wg_smem_attributes<float>();
+        if (rc) return rc;
+        if ((rc = set_wg_smem_attributes<__half>())) return rc;
         if (dev < 64) attr_set[dev] = true;
     }
     // rays per tile: 32 (best gather locality) unless the batch is too small to give every warpgroup a group
@@ -761,16 +789,41 @@ int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool 
     if (grid <= 0) return MVSN_OK;
     const uint8_t* w = static_cast<const uint8_t*>(wimg);
     const int smem = smem_bytes(split), nthreads = threads(split);
-    if (t_stop) {                                         // early ray termination: the ray entry only
-        if (split) render_wg_kernel<true, true, true><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done);
-        else       render_wg_kernel<true, false, true><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done);
-    } else if (split) {
-        if (fast) render_wg_kernel<true, true><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
-        else      render_wg_kernel<false, true><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
-    } else {
-        if (fast) render_wg_kernel<true, false><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
-        else      render_wg_kernel<false, false><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
+    if (half_vol) launch_wg_kernel<__half>(grid, nthreads, smem, stream, sc, io, w, fast, split, t_stop, tiles_done);
+    else          launch_wg_kernel<float>(grid, nthreads, smem, stream, sc, io, w, fast, split, t_stop, tiles_done);
+    MVSN_CUDA_CHECK(cudaGetLastError());
+    return MVSN_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// fp16 volume image: [8][nvox] (planar) or [nvox][8] (channels-last), fp32 or fp16 -> [nvox][8] fp16, rounded as
+// Tensor.half() rounds (__float2half_rn: overflow to inf, subnormals kept; an fp16 source is copied)
+// ------------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void volume_to_half_kernel(const T* __restrict__ src, bool planar, long long nvox, uint4* __restrict__ dst) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nvox; i += (long long)gridDim.x * blockDim.x) {
+        __half h[8];
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const T v = planar ? src[c * nvox + i] : src[8 * i + c];
+            if constexpr (std::is_same<T, __half>::value) h[c] = v;
+            else h[c] = __float2half_rn(v);
+        }
+        uint4 o;
+        o.x = (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16);
+        o.y = (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16);
+        o.z = (uint32_t)__half_as_ushort(h[4]) | ((uint32_t)__half_as_ushort(h[5]) << 16);
+        o.w = (uint32_t)__half_as_ushort(h[6]) | ((uint32_t)__half_as_ushort(h[7]) << 16);
+        dst[i] = o;
     }
+}
+
+int launch_volume_to_half(const void* src, bool src_half, bool src_planar, long long nvox, void* dst, cudaStream_t stream) {
+    const int grid = cdiv(nvox, 256) < 8192 ? cdiv(nvox, 256) : 8192;
+    if (src_half)
+        volume_to_half_kernel<__half><<<grid, 256, 0, stream>>>(static_cast<const __half*>(src), src_planar, nvox, static_cast<uint4*>(dst));
+    else
+        volume_to_half_kernel<float><<<grid, 256, 0, stream>>>(static_cast<const float*>(src), src_planar, nvox, static_cast<uint4*>(dst));
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;
 }

@@ -34,7 +34,9 @@ EXPORTS = [
     "mvsn_render_backward_rays_workspace_bytes", "mvsn_render_backward_rays",
     "mvsn_render_rays_stop",
     "mvsn_render_backward_rays_stop_workspace_bytes", "mvsn_render_backward_rays_stop",
+    "mvsn_volume_to_half", "mvsn_costreg_forward_f16",
 ]
+VOLUME_F16 = 0x100       # OR-ed into RenderScene.mlp_mode (TC modes): volume_dhwc is an fp16 [D,Hp,Wp,8] image
 MAX_PEERS, PEER_HANDLE_BYTES = 16, 64
 BN_BATCH, BN_BATCH_UPDATE, BN_RUNNING = 0, 1, 2
 CONV0_FFMA = 0x100
@@ -82,6 +84,7 @@ def load() -> C.CDLL:
     lib.mvsn_pack_images.argtypes = [vp, ip, ip, ip, vp, vp]
     lib.mvsn_volume_to_channels_last.argtypes = [vp, ip, ip, ip, vp, vp]
     lib.mvsn_volume_from_channels_last.argtypes = [vp, ip, ip, ip, vp, vp]
+    lib.mvsn_volume_to_half.argtypes = [vp, ip, ip, ip, ip, ip, vp, vp]
     lib.mvsn_render_samples.argtypes = [C.POINTER(RenderScene), vp, vp, vp, vp, ip, ip, vp, vp, vp, vp, vp, vp]
     lib.mvsn_render_rays.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), vp, vp, ip, ip,
                                      vp, vp, vp, vp, vp, vp]
@@ -128,6 +131,7 @@ def load() -> C.CDLL:
                                    fp, fp, fp, fp, ip, vp]
     lib.mvsn_adam_step_volume.argtypes = [vp, vp, vp, vp, C.c_longlong, ip, fp, fp, fp, fp, ip, vp]
     lib.mvsn_costreg_forward_bn.argtypes = [C.POINTER(vp), C.POINTER(vp), ip, fp, vp, ip, ip, ip, vp, vp, C.c_size_t, vp]
+    lib.mvsn_costreg_forward_f16.argtypes = lib.mvsn_costreg_forward_bn.argtypes
     lib.mvsn_featurenet_forward_bn.argtypes = [C.POINTER(vp), C.POINTER(vp), ip, fp, vp, ip, ip, ip, vp, vp, C.c_size_t, vp]
     lib.mvsn_make_rays.argtypes = [vp, vp, fp, fp, ip, vp, vp]
     lib.mvsn_make_rays.restype = ip
@@ -139,7 +143,8 @@ def load() -> C.CDLL:
                  "mvsn_peer_buffer_close", "mvsn_peer_buffer_destroy", "mvsn_render_backward", "mvsn_render_backward_tc",
                  "mvsn_render_backward_deterministic", "mvsn_render_backward_rays",
                  "mvsn_render_backward_rays_stop", "mvsn_adam_step",
-                 "mvsn_adam_step_volume", "mvsn_featurenet_forward_bn", "mvsn_costreg_forward_bn"):
+                 "mvsn_adam_step_volume", "mvsn_featurenet_forward_bn", "mvsn_costreg_forward_bn",
+                 "mvsn_volume_to_half", "mvsn_costreg_forward_f16"):
         getattr(lib, name).restype = ip
     _lib = lib
     return lib

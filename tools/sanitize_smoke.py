@@ -3,8 +3,9 @@
 
     compute-sanitizer --tool initcheck python tools/sanitize_smoke.py
 
-K-F FeatureNet, K-A cost volume (the F5 zero border matters for initcheck), K-B CostRegNet (train + eval BN), the four
-K-C render kernels (both entries), the peer sink, the backward kernel + reduce + both Adam kernels, layout helpers."""
+K-F FeatureNet, K-A cost volume (the F5 zero border matters for initcheck), K-B CostRegNet (train + eval BN, fp32 and
+fp16 output), the K-C render kernels (both entries, fp32 and fp16 volume), the peer sink, the backward kernel + reduce +
+both Adam kernels, layout helpers."""
 import os
 import sys
 
@@ -24,6 +25,7 @@ with torch.no_grad():
     if not only or "encoder" in only:
         mvs.eval()(d.imgs_norm, d.proj_mats, sc.near_far, pad=sc.pad)
         mvs.train()
+        mvs(d.imgs_norm, d.proj_mats, sc.near_far, pad=sc.pad, volume_dtype=torch.float16)   # fp16 encoder output
     rays = synthetic.scene_rays(sc)[::3].contiguous().to(dev)
     if not only or "render" in only:
         for mode in (lib.MLP_FP32, lib.MLP_TC_HALF, lib.MLP_TC_SPLIT, lib.MLP_TC_PAIR):
@@ -40,6 +42,23 @@ with torch.no_grad():
                 for t_stop in (0.0, 0.5, 2.0):
                     backend.render_rays(many, vol, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=128,
                                         mlp_mode=mode, t_stop=t_stop, tiles_done=torch.zeros(1, dtype=torch.int64, device=dev))
+                # fp16 volume (MVSN_VOLUME_F16): channels-last in place, then planar through mvsn_volume_to_half; both
+                # entries, the sink and the STOP instantiations
+                for vh in (vol.half(), vol.contiguous().half()):
+                    backend.render_rays(rays, vh, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=24,
+                                        mlp_mode=mode, out=(torch.empty(rays.shape[0], 3, device=dev),
+                                                            torch.empty(rays.shape[0], device=dev)), sink=sink)
+                    backend.render_rays(many, vh, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=128,
+                                        mlp_mode=mode, t_stop=0.5, tiles_done=torch.zeros(1, dtype=torch.int64, device=dev))
+                    xyz_h, _, rd_h, z_h = backend.ray_marcher(rays[:100], N_samples=24)
+                    ndc_h = backend.get_ndc_coordinate(d.pose_source["w2cs"][0], d.pose_source["intrinsics"][0], xyz_h,
+                                                       torch.tensor([sc.W - 1.0, sc.H - 1.0], device=dev),
+                                                       near=sc.near_far[0], far=sc.near_far[1], pad=sc.pad)
+
+                    class AH:
+                        use_color_volume = False
+                    backend.rendering(AH(), d.pose_source, xyz_h, ndc_h, z_h, None, rd_h, volume_feature=vh, imgs=d.imgs_raw,
+                                      network_fn=fn, mlp_mode=mode)
             xyz, _, rd, z = backend.ray_marcher(rays[:100], N_samples=24)
             ndc = backend.get_ndc_coordinate(d.pose_source["w2cs"][0], d.pose_source["intrinsics"][0], xyz,
                                              torch.tensor([sc.W - 1.0, sc.H - 1.0], device=dev), near=sc.near_far[0],
