@@ -153,6 +153,47 @@ int mvsn_render_rays_stop(const mvsn_render_scene* scene, const mvsn_ray_params*
                           const float* rays, const float* t_steps, int N, int S, float t_stop,
                           float* rgb, float* depth, unsigned long long* tiles_done, void* stream);
 
+/* Empty-space skipping.  An occupancy grid holds one bit per cell of the scene's D x Hp x Wp encoding-volume node grid
+ * in NDC: bit c = (d * Hp + y) * Wp + x of the 32-bit word c / 32, least significant bit first,
+ * mvsn_occupancy_bytes(D, Hp, Wp) = 4 * ceil(D * Hp * Wp / 32) bytes (586 KB at 512x640, pad 24).  Cell (d, y, x) with
+ * d < D - 1, y < Hp - 1, x < Wp - 1 spans the nodes d..d+1, y..y+1, x..x+1; the other bits are 0.
+ *
+ * mvsn_build_occupancy evaluates the density at every node (NDC = the node; the world point inverts
+ * utils.get_ndc_coordinate for rp, pad and lindisp included) with the samples entry in MVSN_MLP_TC_SPLIT, sets a cell
+ * when alpha = 1 - exp(-sigma) > 0 at any of its eight corner nodes, then dilates by `dilate` cells (a (2 dilate + 1)^3
+ * box).  scene->mlp_mode must be MVSN_MLP_TC_SPLIT (| MVSN_VOLUME_F16: fp32 and fp16 volumes); scene->white_bkgd is
+ * unused; D, Hp, Wp >= 2; 0 <= dilate <= 8.  bits: mvsn_occupancy_bytes, 4-byte aligned, OVERWRITTEN.  Workspace:
+ * mvsn_build_occupancy_workspace_bytes(D, Hp, Wp) bytes, 16-byte aligned (0 for D, Hp or Wp < 2).  The grid depends on
+ * the volume, the MLP, the source images and cameras and rp: rebuild it after fine-tuning.  Argument errors are
+ * returned before any CUDA call. */
+typedef struct mvsn_occupancy {
+    const uint32_t* bits;       /* device, 4-byte aligned */
+    int D, Hp, Wp;              /* must equal the scene's volume dims */
+} mvsn_occupancy;
+
+size_t mvsn_occupancy_bytes(int D, int Hp, int Wp);
+size_t mvsn_build_occupancy_workspace_bytes(int D, int Hp, int Wp);
+int mvsn_build_occupancy(const mvsn_render_scene* scene, const mvsn_ray_params* rp, int dilate, uint32_t* bits,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
+/* mvsn_render_rays_occ: mvsn_render_rays_stop with empty-space skipping.  A pre-pass marches every ray with the render
+ * kernel's own ray march and NDC and gives each group of rays the range [k_first, k_last] of the tiles that hold a
+ * sample in an occupied cell (a sample outside [0,1]^3 counts as occupied); the group computes only that range, with
+ * the t_stop rule counted in computed tiles, and a group with no occupied sample stores rgb 0 (1 with white_bkgd) and
+ * depth 0 without computing a tile.  Inside the range the arithmetic is mvsn_render_rays_stop's, so a pixel is
+ * bit-identical to the full render whenever the full render's alpha is exactly 0 on every skipped sample; otherwise,
+ * with A = 1 - prod over the skipped leading samples of (1 - alpha), each channel differs by at most A plus the
+ * transmittance left after k_last, plus the t_stop bound.  The grid is a heuristic: these are properties of the scene,
+ * not guarantees.  An all-ones grid with t_stop gives exactly mvsn_render_rays_stop's results.  tiles_done as there.
+ * Modes MVSN_MLP_TC_HALF / TC_PAIR / TC_SPLIT.  Workspace (the range table): mvsn_render_rays_occ_workspace_bytes(N, S)
+ * bytes, 16-byte aligned.  Argument errors are returned before any CUDA call: those of mvsn_render_rays_stop, a NULL or
+ * misaligned grid, grid dims other than the scene's (MVSN_EBADSHAPE), a small or misaligned workspace. */
+size_t mvsn_render_rays_occ_workspace_bytes(int N, int S);
+int mvsn_render_rays_occ(const mvsn_render_scene* scene, const mvsn_ray_params* rp,
+                         const float* rays, const float* t_steps, int N, int S, float t_stop,
+                         const mvsn_occupancy* occupancy, float* rgb, float* depth, unsigned long long* tiles_done,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
 /* Ray generation for one camera (replaces: data/ray_utils.get_rays, data/ray_utils.py:32-53, and the notebooks'
  * `torch.cat([rays_o, rays_d, near, far])`): directions [n,3] = get_ray_directions(H, W, focal) in camera coordinates
  * (resident on the device, they depend on the intrinsics only), c2w = the first three rows of the camera-to-world matrix,

@@ -1042,10 +1042,78 @@ def _ordered_named_params(network_fn):
 
 
 _tsteps = {}
+_occ_workspace = {}          # per device: the range table of render_rays(occupancy=), grown to the largest batch
+
+
+class Occupancy:
+    """An occupancy grid of a scene's density for empty-space skipping (`render_rays(..., occupancy=)`): one bit per cell
+    of the encoding volume's D x Hp x Wp node grid in NDC (`bits`, int32 words, see mvsn_build_occupancy), and the
+    geometry it was built for -- the rays' NDC mapping must be the same (near_far, pad, lindisp) for it to apply."""
+
+    def __init__(self, bits, D, Hp, Wp, near_far, pad, lindisp, dilate):
+        self.bits, self.D, self.Hp, self.Wp = bits, int(D), int(Hp), int(Wp)
+        self.near_far, self.pad, self.lindisp, self.dilate = (float(near_far[0]), float(near_far[1])), float(pad), \
+            bool(lindisp), int(dilate)
+
+    def cells(self):
+        """bool [D, Hp, Wp]: cell (d, y, x) occupied (the last slab of each axis is always False)."""
+        n = self.D * self.Hp * self.Wp
+        shifts = torch.arange(32, dtype=torch.int32, device=self.bits.device)
+        return ((self.bits.view(-1, 1) >> shifts) & 1).bool().reshape(-1)[:n].view(self.D, self.Hp, self.Wp)
+
+    def fraction(self):
+        """occupied cells / all (D - 1) (Hp - 1) (Wp - 1) cells"""
+        return float(self.cells().sum()) / ((self.D - 1) * (self.Hp - 1) * (self.Wp - 1))
+
+    def _grid(self):
+        return _lib.OccupancyGrid(self.bits.data_ptr(), self.D, self.Hp, self.Wp)
+
+
+def build_occupancy(volume_feature, imgs, pose_ref, network_fn, near_far, pad, lindisp=False, dilate=1):
+    """The occupancy grid of a scene for `render_rays(..., occupancy=)` (mvsn_build_occupancy): sigma at every node of the
+    volume's grid (the split tensor-core MLP, the node as the sample's NDC, the world point from inverting
+    get_ndc_coordinate with `near_far` / `pad` / `lindisp`), a cell occupied when alpha > 0 at any of its eight corners,
+    then dilated by `dilate` cells (0..8).  fp32 and fp16 volumes.  Returns an `Occupancy`.
+
+    The grid depends on the volume, the MLP, the source images and cameras: it is cached on their version counters (a
+    repeated call returns the same object), so call build_occupancy again after fine-tuning -- an `Occupancy` held from
+    before describes the old scene."""
+    dilate = int(dilate)
+    if not 0 <= dilate <= 8:
+        raise RuntimeError(f"build_occupancy: dilate={dilate} must be in 0..8")
+    owner = volume_feature.feat_volume if isinstance(volume_feature, nn.Module) else volume_feature
+    if not owner.is_cuda:
+        raise RuntimeError("build_occupancy: the encoding volume must be a CUDA tensor; mvsnerf_b200 has no CPU path")
+    params = network_fn.ordered_params()
+    tensors = [owner, imgs, pose_ref["w2cs"], pose_ref["intrinsics"]] + list(params)
+    args = (float(near_far[0]), float(near_far[1]), float(pad), bool(lindisp), dilate)
+    hit = _cache.get("occupancy")
+    if hit is not None and hit[1] == args and len(hit[0]) == len(tensors) and \
+            all(r() is t and v == t._version for (r, v), t in zip(hit[0], tensors)):
+        cache_stats["hit"] += 1
+        return hit[2]
+    cache_stats["miss"] += 1
+    lib = _lib.load()
+    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, False, _lib.MLP_TC_SPLIT, half_ok=True)
+    dev = owner.device
+    rp = _lib.RayParams(args[0], args[1], args[2], int(args[3]))
+    bits = torch.empty(lib.mvsn_occupancy_bytes(sc.D, sc.Hp, sc.Wp) // 4, dtype=torch.int32, device=dev)
+    need = lib.mvsn_build_occupancy_workspace_bytes(sc.D, sc.Hp, sc.Wp)
+    if need == 0:
+        raise RuntimeError(f"build_occupancy: volume {sc.D}x{sc.Hp}x{sc.Wp} (every dim >= 2)")
+    ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.mvsn_build_occupancy(C.byref(sc), C.byref(rp), dilate, _lib.ptr(bits), _lib.ptr(ws), need,
+                                            _lib.stream_ptr()), "mvsn_build_occupancy")
+    del keep
+    occ = Occupancy(bits, sc.D, sc.Hp, sc.Wp, near_far, pad, lindisp, dilate)
+    _cache["occupancy"] = ([(weakref.ref(t), t._version) for t in tensors], args, occ)
+    return occ
 
 
 def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad, N_samples=128,
-                white_bkgd=False, lindisp=False, mlp_mode=None, out=None, sink=None, t_stop=None, tiles_done=None):
+                white_bkgd=False, lindisp=False, mlp_mode=None, out=None, sink=None, t_stop=None, tiles_done=None,
+                occupancy=None):
     """Fused-caller entry: one launch renders all `rays` [N,8] = (o, d, near, far).
 
     Replaces the notebooks' per-chunk loop `ray_marcher -> get_ndc_coordinate -> rendering`
@@ -1062,11 +1130,30 @@ def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
     each channel differs from the full render by less than t_stop (t_stop = 0: bit-identical).  `tiles_done`: an
     optional CUDA int64 tensor [1] the number of computed 64-sample tiles is added to.  Not combinable with `sink`.
 
+    `occupancy` (an `Occupancy` from build_occupancy for this scene, near_far, pad and lindisp; tensor-core modes):
+    empty-space skipping (mvsn_render_rays_occ) -- each group of rays computes only the tiles from its first to its last
+    sample in an occupied cell, and a group with none stores rgb 0 (1 with white_bkgd) and depth 0.  A pixel is
+    bit-identical to the full render whenever the full render's alpha is exactly 0 on every skipped sample; the grid is a
+    heuristic (DESIGN §4 K-C).  Composes with `t_stop` (without it the call runs with t_stop = 0, which never stops);
+    `tiles_done` works with either.  Not combinable with `sink`.
+
     A float16 `volume_feature` is read as fp16 in the tensor-core modes (half the resident bytes): the result is
     bit-identical to rendering `volume.float()`.  Channels-last storage (MVSNet.forward(..., volume_dtype=torch.float16),
     or `.half()` of an fp32 MVSNet volume) is read in place; other layouts are converted once per tensor version."""
     lib = _lib.load()
     mode = DEFAULT_MLP_MODE if mlp_mode is None else mlp_mode
+    if occupancy is not None:
+        if sink is not None:
+            raise RuntimeError("render_rays: occupancy cannot be combined with sink (peer frame assembly)")
+        if mode == _lib.MLP_FP32:
+            raise RuntimeError("render_rays: occupancy needs a tensor-core mlp_mode (MLP_TC_HALF / TC_PAIR / TC_SPLIT)")
+        if not isinstance(occupancy, Occupancy):
+            raise RuntimeError("render_rays: occupancy must be an Occupancy from build_occupancy")
+        if occupancy.near_far != (float(near_far[0]), float(near_far[1])) or occupancy.pad != float(pad) or \
+                occupancy.lindisp != bool(lindisp):
+            raise RuntimeError("render_rays: the occupancy grid was built for another near_far / pad / lindisp")
+        if t_stop is None:
+            t_stop = 0.0
     if t_stop is not None:
         t_stop = float(t_stop)
         if sink is not None:
@@ -1093,7 +1180,20 @@ def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
         rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
         depth = torch.empty(N, dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        if t_stop is not None:
+        if occupancy is not None:
+            if occupancy.bits.device != dev:
+                raise RuntimeError(f"render_rays: the occupancy grid is on {occupancy.bits.device}, the rays on {dev}")
+            need = lib.mvsn_render_rays_occ_workspace_bytes(N, S)
+            ws = _occ_workspace.get(dev)
+            if ws is None or ws.numel() < need:
+                ws = torch.empty(need, dtype=torch.uint8, device=dev)
+                _occ_workspace[dev] = ws
+            grid = occupancy._grid()
+            _lib.check(lib.mvsn_render_rays_occ(C.byref(sc), C.byref(rp), _lib.ptr(rays), _lib.ptr(t_steps), N, S, t_stop,
+                                                C.byref(grid), _lib.ptr(rgb), _lib.ptr(depth), _lib.ptr(tiles_done),
+                                                _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
+                       "mvsn_render_rays_occ")
+        elif t_stop is not None:
             _lib.check(lib.mvsn_render_rays_stop(C.byref(sc), C.byref(rp), _lib.ptr(rays), _lib.ptr(t_steps), N, S,
                                                  t_stop, _lib.ptr(rgb), _lib.ptr(depth), _lib.ptr(tiles_done),
                                                  _lib.stream_ptr()),

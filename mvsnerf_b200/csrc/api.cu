@@ -312,24 +312,36 @@ int mvsn_render_rays(const mvsn_render_scene* scene, const mvsn_ray_params* rp, 
     return render_rays_impl(scene, rp, rays, t_steps, N, S, rgb, depth, weights, alpha, input_feat, nullptr, stream);
 }
 
-int mvsn_render_rays_stop(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const float* rays,
-                          const float* t_steps, int N, int S, float t_stop, float* rgb, float* depth,
-                          unsigned long long* tiles_done, void* stream) {
-    MVSN_RANGE("mvsn_render_rays_stop");
+// mvsn_render_rays_stop and, with `occ`, mvsn_render_rays_occ (`what`: the entry's name for messages)
+static int render_rays_stop_entry(const char* what, const mvsn_render_scene* scene, const mvsn_ray_params* rp,
+                                  const float* rays, const float* t_steps, int N, int S, float t_stop,
+                                  const mvsn_occupancy* occ, float* rgb, float* depth, unsigned long long* tiles_done,
+                                  void* workspace, size_t workspace_bytes, void* stream) {
     SceneDev sc;
     int rc = make_scene(scene, sc);
     if (rc) return rc;
-    MVSN_REQUIRE(rp != nullptr, MVSN_ENULL, "mvsn_render_rays_stop: ray params NULL");
-    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "mvsn_render_rays_stop: N=%d S=%d", N, S);
-    MVSN_REQUIRE(rays && t_steps && rgb && depth, MVSN_ENULL, "mvsn_render_rays_stop: NULL required pointer");
-    MVSN_REQUIRE(t_stop >= 0.f, MVSN_EBADSHAPE, "mvsn_render_rays_stop: t_stop=%g must be >= 0 (not NaN)", (double)t_stop);
+    MVSN_REQUIRE(rp != nullptr, MVSN_ENULL, "%s: ray params NULL", what);
+    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "%s: N=%d S=%d", what, N, S);
+    MVSN_REQUIRE(rays && t_steps && rgb && depth, MVSN_ENULL, "%s: NULL required pointer", what);
+    MVSN_REQUIRE(t_stop >= 0.f, MVSN_EBADSHAPE, "%s: t_stop=%g must be >= 0 (not NaN)", what, (double)t_stop);
     const int mode = mlp_mode_of(scene);
     MVSN_REQUIRE(mode == MVSN_MLP_TC_HALF || mode == MVSN_MLP_TC_PAIR || mode == MVSN_MLP_TC_SPLIT,
-                 MVSN_EUNSUPPORTED, "mvsn_render_rays_stop: mlp_mode %d has no early ray termination (tensor-core modes only)",
+                 MVSN_EUNSUPPORTED, "%s: mlp_mode %d has no early ray termination (tensor-core modes only)", what,
                  scene->mlp_mode);
     MVSN_REQUIRE(aligned16(rays), MVSN_EALIGN, "rays must be 16-byte aligned");
-    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(tiles_done) % 8 == 0, MVSN_EALIGN,
-                 "mvsn_render_rays_stop: tiles_done must be 8-byte aligned");
+    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(tiles_done) % 8 == 0, MVSN_EALIGN, "%s: tiles_done must be 8-byte aligned", what);
+    if (occ) {
+        MVSN_REQUIRE(occ->bits != nullptr, MVSN_ENULL, "%s: occupancy->bits is NULL", what);
+        MVSN_REQUIRE(reinterpret_cast<uintptr_t>(occ->bits) % 4 == 0, MVSN_EALIGN, "%s: occupancy->bits must be 4-byte aligned",
+                     what);
+        MVSN_REQUIRE(occ->D == scene->D && occ->Hp == scene->Hp && occ->Wp == scene->Wp && occ->D >= 2 && occ->Hp >= 2 &&
+                     occ->Wp >= 2, MVSN_EBADSHAPE, "%s: occupancy grid %dx%dx%d does not match the scene's volume %dx%dx%d",
+                     what, occ->D, occ->Hp, occ->Wp, scene->D, scene->Hp, scene->Wp);
+        MVSN_REQUIRE(workspace != nullptr, MVSN_ENULL, "%s: workspace is NULL", what);
+        MVSN_REQUIRE(aligned16(workspace), MVSN_EALIGN, "%s: workspace must be 16-byte aligned", what);
+        MVSN_REQUIRE(workspace_bytes >= occupancy_ranges_bytes(N), MVSN_EWORKSPACE, "%s: workspace needs %zu bytes, got %zu",
+                     what, occupancy_ranges_bytes(N), workspace_bytes);
+    }
     if (N == 0) return MVSN_OK;
     RenderIO io{};
     io.rays = rays; io.t_steps = t_steps;
@@ -337,7 +349,58 @@ int mvsn_render_rays_stop(const mvsn_render_scene* scene, const mvsn_ray_params*
     io.rgb = rgb; io.depth = depth;
     io.rg = make_ray_gen(scene, rp);
     return launch_render_wg(sc, io, true, mode == MVSN_MLP_TC_SPLIT, scene->mlp_packed, (cudaStream_t)stream,
-                            &t_stop, tiles_done, half_volume(scene));
+                            &t_stop, tiles_done, half_volume(scene), occ ? occ->bits : nullptr,
+                            occ ? static_cast<int2*>(workspace) : nullptr);
+}
+
+int mvsn_render_rays_stop(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const float* rays,
+                          const float* t_steps, int N, int S, float t_stop, float* rgb, float* depth,
+                          unsigned long long* tiles_done, void* stream) {
+    MVSN_RANGE("mvsn_render_rays_stop");
+    return render_rays_stop_entry("mvsn_render_rays_stop", scene, rp, rays, t_steps, N, S, t_stop, nullptr, rgb, depth,
+                                  tiles_done, nullptr, 0, stream);
+}
+
+size_t mvsn_render_rays_occ_workspace_bytes(int N, int S) {
+    return N >= 0 && S > 0 ? occupancy_ranges_bytes(N) : 0;
+}
+
+int mvsn_render_rays_occ(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const float* rays,
+                         const float* t_steps, int N, int S, float t_stop, const mvsn_occupancy* occupancy, float* rgb,
+                         float* depth, unsigned long long* tiles_done, void* workspace, size_t workspace_bytes,
+                         void* stream) {
+    MVSN_RANGE("mvsn_render_rays_occ");
+    MVSN_REQUIRE(occupancy != nullptr, MVSN_ENULL, "mvsn_render_rays_occ: occupancy is NULL");
+    return render_rays_stop_entry("mvsn_render_rays_occ", scene, rp, rays, t_steps, N, S, t_stop, occupancy, rgb, depth,
+                                  tiles_done, workspace, workspace_bytes, stream);
+}
+
+size_t mvsn_occupancy_bytes(int D, int Hp, int Wp) {
+    return D > 0 && Hp > 0 && Wp > 0 ? occupancy_words(D, Hp, Wp) * 4 : 0;
+}
+
+size_t mvsn_build_occupancy_workspace_bytes(int D, int Hp, int Wp) { return occupancy_workspace_bytes(D, Hp, Wp); }
+
+int mvsn_build_occupancy(const mvsn_render_scene* scene, const mvsn_ray_params* rp, int dilate, uint32_t* bits,
+                         void* workspace, size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_build_occupancy");
+    SceneDev sc;
+    int rc = make_scene(scene, sc);
+    if (rc) return rc;
+    MVSN_REQUIRE(rp && bits && workspace, MVSN_ENULL, "mvsn_build_occupancy: NULL argument");
+    MVSN_REQUIRE(mlp_mode_of(scene) == MVSN_MLP_TC_SPLIT, MVSN_EUNSUPPORTED,
+                 "mvsn_build_occupancy: scene->mlp_mode %d (the MVSN_MLP_TC_SPLIT image, optionally | MVSN_VOLUME_F16)",
+                 scene->mlp_mode);
+    MVSN_REQUIRE(scene->D >= 2 && scene->Hp >= 2 && scene->Wp >= 2, MVSN_EBADSHAPE,
+                 "mvsn_build_occupancy: volume %dx%dx%d (every dim >= 2)", scene->D, scene->Hp, scene->Wp);
+    MVSN_REQUIRE(dilate >= 0 && dilate <= 8, MVSN_EBADSHAPE, "mvsn_build_occupancy: dilate=%d (0..8)", dilate);
+    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(bits) % 4 == 0, MVSN_EALIGN, "mvsn_build_occupancy: bits must be 4-byte aligned");
+    MVSN_REQUIRE(aligned16(workspace), MVSN_EALIGN, "mvsn_build_occupancy: workspace must be 16-byte aligned");
+    const size_t need = occupancy_workspace_bytes(scene->D, scene->Hp, scene->Wp);
+    MVSN_REQUIRE(workspace_bytes >= need, MVSN_EWORKSPACE, "mvsn_build_occupancy: workspace needs %zu bytes, got %zu", need,
+                 workspace_bytes);
+    return build_occupancy(sc, make_ray_gen(scene, rp), scene->mlp_packed, half_volume(scene), dilate, bits, workspace,
+                           (cudaStream_t)stream);
 }
 
 int mvsn_render_rays_to_peers(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const float* rays,

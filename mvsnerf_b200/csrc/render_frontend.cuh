@@ -68,9 +68,20 @@ __device__ __forceinline__ void store_pixel(const RenderIO& io, int ray, float r
 int launch_render_fp32(const SceneDev& sc, const RenderIO& io, bool fast, const float* wts, cudaStream_t stream);
 // tensor-core modes (render_wg.cu): split = MVSN_MLP_TC_SPLIT, otherwise the fp16-operand modes.  t_stop != NULL
 // (fast only): early ray termination at transmittance *t_stop; tiles_done (may be NULL) += the tiles computed.
-// half_vol: sc.vol is an fp16 [D,Hp,Wp,8] image (MVSN_VOLUME_F16)
+// half_vol: sc.vol is an fp16 [D,Hp,Wp,8] image (MVSN_VOLUME_F16).  occ_bits (with t_stop; empty-space skipping): an
+// occupancy grid of the scene's D x Hp x Wp cells; its per-group tile ranges go to `ranges` (occupancy_ranges_bytes(N)).
 int launch_render_wg(const SceneDev& sc, const RenderIO& io, bool fast, bool split, const void* wimg, cudaStream_t stream,
-                     const float* t_stop = nullptr, unsigned long long* tiles_done = nullptr, bool half_vol = false);
+                     const float* t_stop = nullptr, unsigned long long* tiles_done = nullptr, bool half_vol = false,
+                     const uint32_t* occ_bits = nullptr, int2* ranges = nullptr);
+// occupancy.cu: the grid (mvsn_build_occupancy; wimg_split = the MVSN_MLP_TC_SPLIT image) and the range pre-pass of a
+// ray launch (io.rays_per_tile set; precise = the split mode's NDC arithmetic)
+size_t occupancy_words(int D, int Hp, int Wp);
+size_t occupancy_workspace_bytes(int D, int Hp, int Wp);
+size_t occupancy_ranges_bytes(int N);
+int build_occupancy(const SceneDev& sc, const RayGenDev& rg, const void* wimg_split, bool half_vol, int dilate,
+                    uint32_t* bits, void* workspace, cudaStream_t stream);
+int launch_occupancy_ranges(const SceneDev& sc, const RenderIO& io, bool precise, const uint32_t* bits, int2* ranges,
+                            cudaStream_t stream);
 // fp16 [D,Hp,Wp,8] image of a planar [8,D,Hp,Wp] or channels-last volume, fp32 or fp16, rounded with __float2half_rn
 int launch_volume_to_half(const void* src, bool src_half, bool src_planar, long long nvox, void* dst, cudaStream_t stream);
 size_t mlp_wg_packed_bytes(bool split);

@@ -115,6 +115,24 @@ __device__ __forceinline__ void stop_wait(WgStop* ss, int pass) {
 }
 __device__ __forceinline__ int2 stop_plan(const WgStop* ss, int pass, int w) { return ss->plan[pass & (STOP_SLOTS - 1)][w]; }
 __device__ __forceinline__ bool stop_busy(const WgStop* ss, int pass, int w) { return stop_plan(ss, pass, w).x >= 0; }
+__device__ __forceinline__ const int2* range_table(const int2* ranges) { return ranges; }
+// the tiles [first, last] of group g that hold an occupied sample (empty-space skipping: the range table the pre-pass
+// wrote; last < first: none); [0, NT - 1] without a table
+__device__ __forceinline__ int2 stop_range(const int2* ranges, int g, int NT) {
+    return ranges ? __ldg(ranges + g) : make_int2(0, NT - 1);
+}
+// the first plan (group, first tile) of the next group of the CTA's list with a non-empty range; (-1, 0) when none is
+// left.  next_index() hands out the list's indices (stop_group is increasing in them).
+template <typename NextIndex>
+__device__ __forceinline__ int2 stop_take(const int2* ranges, NextIndex next_index, int G, int NT) {
+#pragma unroll 1
+    while (true) {
+        const int g = stop_group(next_index());
+        if (g >= G) return make_int2(-1, 0);
+        const int2 r = stop_range(ranges, g, NT);
+        if (r.y >= r.x) return make_int2(g, r.x);
+    }
+}
 
 __device__ __forceinline__ uint32_t pack_h2_rn(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
@@ -338,8 +356,9 @@ __device__ __forceinline__ void front_end(const SceneDev& sc, const Cams& cams, 
 }
 
 // STOP: the state a consumer carries from pass to pass -- the verdict of the tile composited last (warp 0: every valid
-// ray of the group has cT < t_stop), no work left, the current tile is its group's last, tiles computed
-template <bool STOP> struct StopRegs { bool verdict = false, idle = false, last = false; uint32_t ncomp = 0; };
+// ray of the group has cT < t_stop), no work left, the current tile is its group's last, the current tile is its
+// group's first (the previous one was a group's last), tiles computed
+template <bool STOP> struct StopRegs { bool verdict = false, idle = false, last = false, first = true; uint32_t ncomp = 0; };
 template <> struct StopRegs<false> { static constexpr bool last = false; };
 
 // STOP (early ray termination, FAST only): after compositing tile k of a group, if every valid ray of the group has
@@ -348,12 +367,18 @@ template <> struct StopRegs<false> { static constexpr bool last = false; };
 // start of pass p: the next tile of its group, or the next group of the CTA's list (a shared counter, in order of
 // demand), or idle.  Tile k + 2 depends only on the verdicts up to tile k - 1, so every plan is known two passes ahead
 // and the producer fills a slot as soon as its consumer releases it, as without STOP.  Without STOP the kernel is the
-// one it always was (t_stop and tiles_done are unused).
+// one it always was (t_stop, tiles_done and ranges are unused).
+// STOP with a range table (empty-space skipping, from occ_ranges_kernel): group g is computed over its tiles
+// [ranges[g].x, ranges[g].y] only -- its first plan starts at .x, its last tile is .y, the t_stop rule counts computed
+// tiles -- and a group with an empty range is not handed out (the pre-pass stored its pixels).  Null: [0, NT - 1].
+// Only the STOP instantiations take the table (Table = const int2*, read through range_table inside STOP code): the
+// others keep their five parameters, because one more kernel parameter alone changes the split kernels' register
+// allocation.
 // VT = __half: the encoding volume is stored as fp16 (sc.vol points at halves); only the volume gather changes.
-template <bool FAST, bool SPLIT, bool STOP = false, typename VT = float>
+template <bool FAST, bool SPLIT, bool STOP = false, typename VT = float, typename... Table>
 __global__ void __launch_bounds__(wg::threads(SPLIT), 1)
 render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict__ wimg, float t_stop,
-                 unsigned long long* tiles_done) {
+                 unsigned long long* tiles_done, Table... table) {
     using namespace wg;
     constexpr int NS = nstage(SPLIT), THREADS = threads(SPLIT);
     extern __shared__ uint8_t smem_raw[];
@@ -373,13 +398,16 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             const int G0 = (io.N + io.rays_per_tile - 1) / io.rays_per_tile;
             const int NT0 = (io.S + wg::ROWS / io.rays_per_tile - 1) / (wg::ROWS / io.rays_per_tile);
             for (int i = 0; i < STOP_SLOTS; ++i) mbar_init(&ss->dec[i], NWG);
-            int next = NWG;                              // passes 0 and 1: first groups, then their tile 1 (or the next group)
+            const int2* ranges = range_table(table...);
+            int next = 0;                               // passes 0 and 1: first groups, then their next tile (or the next group)
+            auto take = [&]() { return next++; };
             for (int w = 0; w < NWG; ++w) {
-                const int g0 = stop_group(w) < G0 ? stop_group(w) : -1;
-                ss->plan[0][w] = make_int2(g0, 0);
-                int2 p1 = make_int2(g0, 1);
-                if (g0 >= 0 && NT0 == 1) { const int gn = stop_group(next++); p1 = make_int2(gn < G0 ? gn : -1, 0); }
-                ss->plan[1][w] = g0 < 0 ? make_int2(-1, 0) : p1;
+                const int2 p0 = stop_take(ranges, take, G0, NT0);
+                int2 p1 = make_int2(-1, 0);
+                if (p0.x >= 0)
+                    p1 = p0.y + 1 <= stop_range(ranges, p0.x, NT0).y ? make_int2(p0.x, p0.y + 1) : stop_take(ranges, take, G0, NT0);
+                ss->plan[0][w] = p0;
+                ss->plan[1][w] = p1;
             }
             ss->next = next;
         }
@@ -517,17 +545,18 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                 for (int c = 0; c < NCHUNK; ++c) { acquire(); release(); }
                 continue;
             }
-            // from the plan of pass + 1, (g, k): tile k + 1 of g is skipped iff k + 1 == NT or the verdict of tile k - 2
-            // (this consumer's last composited tile) says stop
+            // from the plan of pass + 1, (g, k): tile k + 1 of g is skipped iff k is the last of g's range (NT - 1 without
+            // a range table) or the verdict of tile k - 2 (this consumer's last composited tile, if it is one of g's)
+            // says stop
             if (t == 0) {
                 const int2 p1 = stop_plan(ss, pass + 1, wgi);
                 int2 nx = make_int2(-1, 0);
                 if (p1.x >= 0) {
+                    const int2* ranges = range_table(table...);
+                    const int2 r = stop_range(ranges, p1.x, NT);
                     nx = make_int2(p1.x, p1.y + 1);
-                    if (p1.y + 1 >= NT || (p1.y >= 2 && sr.verdict)) {
-                        const int gn = stop_group(atomicAdd(&ss->next, 1));
-                        nx = make_int2(gn < G ? gn : -1, 0);
-                    }
+                    if (p1.y + 1 > r.y || (p1.y >= r.x + 2 && sr.verdict))
+                        nx = stop_take(ranges, [&]() { return atomicAdd(&ss->next, 1); }, G, NT);
                 }
                 ss->plan[(pass + 2) & (STOP_SLOTS - 1)][wgi] = nx;
                 mbar_arrive(&ss->dec[(pass + 2) & (STOP_SLOTS - 1)]);
@@ -700,7 +729,11 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         // the first RT threads walk their ray's SP samples of this tile front to back -- the reference's
         // sequential cumprod order
         if (t < RT) {
-            if (tile == 0) { cT = 1.f; c0 = c1 = c2 = c3 = c4 = 0.f; }
+            if constexpr (STOP) {                        // the group's first tile: the first of its range
+                if (sr.first) { cT = 1.f; c0 = c1 = c2 = c3 = c4 = 0.f; }
+            } else {
+                if (tile == 0) { cT = 1.f; c0 = c1 = c2 = c3 = c4 = 0.f; }
+            }
             const int cray = grp * RT + t;
             if (cray < N) {
                 float znear = 0.f, zfar = 0.f;
@@ -728,6 +761,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         }
         if constexpr (STOP) {                            // rays past the batch end (and lanes >= RT) count as stopped
             if (t < 32) sr.verdict = __all_sync(0xffffffffu, t >= RT || grp * RT + t >= N || cT < t_stop);
+            sr.first = sr.last;
         }
     }
     if constexpr (STOP) {
@@ -743,20 +777,21 @@ static int set_wg_smem_attributes() {
     MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, false, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false)));
     MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
     MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, true, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
-    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false, true, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         smem_bytes(false) + STOP_BYTES));
-    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, true, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         smem_bytes(true) + STOP_BYTES));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false, true, VT, const int2*>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false) + STOP_BYTES));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, true, VT, const int2*>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true) + STOP_BYTES));
     return MVSN_OK;
 }
 
 template <typename VT>
 static void launch_wg_kernel(int grid, int nthreads, int smem, cudaStream_t stream, const SceneDev& sc, const RenderIO& io,
-                             const uint8_t* w, bool fast, bool split, const float* t_stop, unsigned long long* tiles_done) {
+                             const uint8_t* w, bool fast, bool split, const float* t_stop, unsigned long long* tiles_done,
+                             const int2* ranges) {
     using namespace wg;
     if (t_stop) {                                         // early ray termination: the ray entry only
-        if (split) render_wg_kernel<true, true, true, VT><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done);
-        else       render_wg_kernel<true, false, true, VT><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done);
+        if (split) render_wg_kernel<true, true, true, VT, const int2*><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
+        else       render_wg_kernel<true, false, true, VT, const int2*><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
     } else if (split) {
         if (fast) render_wg_kernel<true, true, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
         else      render_wg_kernel<false, true, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
@@ -767,7 +802,8 @@ static void launch_wg_kernel(int grid, int nthreads, int smem, cudaStream_t stre
 }
 
 int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool split, const void* wimg, cudaStream_t stream,
-                     const float* t_stop, unsigned long long* tiles_done, bool half_vol) {
+                     const float* t_stop, unsigned long long* tiles_done, bool half_vol, const uint32_t* occ_bits,
+                     int2* ranges) {
     using namespace wg;
     RenderIO io = io_in;
     static bool attr_set[64] = {false};                   // once per device, not per launch
@@ -789,8 +825,15 @@ int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool 
     if (grid <= 0) return MVSN_OK;
     const uint8_t* w = static_cast<const uint8_t*>(wimg);
     const int smem = smem_bytes(split), nthreads = threads(split);
-    if (half_vol) launch_wg_kernel<__half>(grid, nthreads, smem, stream, sc, io, w, fast, split, t_stop, tiles_done);
-    else          launch_wg_kernel<float>(grid, nthreads, smem, stream, sc, io, w, fast, split, t_stop, tiles_done);
+    if (occ_bits) {                                       // empty-space skipping: the range pre-pass at this launch's rt
+        if (!t_stop || !ranges) { set_error("launch_render_wg: an occupancy grid needs t_stop and a range table"); return MVSN_EBADSHAPE; }
+        const int rc = launch_occupancy_ranges(sc, io, split, occ_bits, ranges, stream);
+        if (rc) return rc;
+    } else {
+        ranges = nullptr;
+    }
+    if (half_vol) launch_wg_kernel<__half>(grid, nthreads, smem, stream, sc, io, w, fast, split, t_stop, tiles_done, ranges);
+    else          launch_wg_kernel<float>(grid, nthreads, smem, stream, sc, io, w, fast, split, t_stop, tiles_done, ranges);
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;
 }

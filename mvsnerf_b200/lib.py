@@ -35,6 +35,8 @@ EXPORTS = [
     "mvsn_render_rays_stop",
     "mvsn_render_backward_rays_stop_workspace_bytes", "mvsn_render_backward_rays_stop",
     "mvsn_volume_to_half", "mvsn_costreg_forward_f16",
+    "mvsn_occupancy_bytes", "mvsn_build_occupancy_workspace_bytes", "mvsn_build_occupancy",
+    "mvsn_render_rays_occ_workspace_bytes", "mvsn_render_rays_occ",
 ]
 VOLUME_F16 = 0x100       # OR-ed into RenderScene.mlp_mode (TC modes): volume_dhwc is an fp16 [D,Hp,Wp,8] image
 MAX_PEERS, PEER_HANDLE_BYTES = 16, 64
@@ -61,6 +63,10 @@ class RenderGrads(C.Structure):
 
 class RayParams(C.Structure):
     _fields_ = [("ndc_near", C.c_float), ("ndc_far", C.c_float), ("pad", C.c_float), ("lindisp", C.c_int)]
+
+
+class OccupancyGrid(C.Structure):
+    _fields_ = [("bits", C.c_void_p), ("D", C.c_int), ("Hp", C.c_int), ("Wp", C.c_int)]
 
 
 _lib = None
@@ -91,6 +97,14 @@ def load() -> C.CDLL:
     lib.mvsn_render_rays_stop.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), vp, vp, ip, ip, fp,
                                           vp, vp, vp, vp]
     lib.mvsn_render_rays_stop.restype = ip
+    for name in ("mvsn_occupancy_bytes", "mvsn_build_occupancy_workspace_bytes"):
+        getattr(lib, name).restype = C.c_size_t
+        getattr(lib, name).argtypes = [ip, ip, ip]
+    lib.mvsn_build_occupancy.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), ip, vp, vp, C.c_size_t, vp]
+    lib.mvsn_render_rays_occ_workspace_bytes.restype = C.c_size_t
+    lib.mvsn_render_rays_occ_workspace_bytes.argtypes = [ip, ip]
+    lib.mvsn_render_rays_occ.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), vp, vp, ip, ip, fp,
+                                         C.POINTER(OccupancyGrid), vp, vp, vp, vp, C.c_size_t, vp]
     lib.mvsn_cost_volume_workspace_bytes.restype = C.c_size_t
     lib.mvsn_cost_volume_workspace_bytes.argtypes = [ip, ip, ip]
     lib.mvsn_build_cost_volume.argtypes = [vp, vp, vp, vp, ip, ip, ip, ip, ip, vp, vp, vp, C.c_size_t, vp]
@@ -144,7 +158,7 @@ def load() -> C.CDLL:
                  "mvsn_render_backward_deterministic", "mvsn_render_backward_rays",
                  "mvsn_render_backward_rays_stop", "mvsn_adam_step",
                  "mvsn_adam_step_volume", "mvsn_featurenet_forward_bn", "mvsn_costreg_forward_bn",
-                 "mvsn_volume_to_half", "mvsn_costreg_forward_f16"):
+                 "mvsn_volume_to_half", "mvsn_costreg_forward_f16", "mvsn_build_occupancy", "mvsn_render_rays_occ"):
         getattr(lib, name).restype = ip
     _lib = lib
     return lib

@@ -172,19 +172,19 @@ class FrameWriter:
 
 
 def render_video(c2ws, directions, volume_feature, imgs, pose_ref, network_fn, near_far, pad, writer=None,
-                 N_samples=128, white_bkgd=False, lindisp=False, mlp_mode=None, t_stop=None):
+                 N_samples=128, white_bkgd=False, lindisp=False, mlp_mode=None, t_stop=None, occupancy=None):
     """The free-viewpoint loop of renderer_video.ipynb (cell "DTU video rendering", raw lines 775-786 hold its
     settings): for every target pose build the rays (get_rays), render the whole frame with ONE fused launch and
     hand the pixels to `writer` (a FrameWriter) or collect them.  Returns the list of (rgb, depth) device tensors
-    when no writer is given, else the number of frames submitted.  `t_stop`: early ray termination (see
-    backend.render_rays)."""
+    when no writer is given, else the number of frames submitted.  `t_stop`: early ray termination; `occupancy`:
+    empty-space skipping with a grid from backend.build_occupancy, which serves every pose (see backend.render_rays)."""
     H, W = directions.shape[:2]
     frames = []
     for i, c2w in enumerate(c2ws):
         rays = camera_rays(directions, c2w, near_far[0], near_far[1])
         rgb, depth = backend.render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
                                          N_samples=N_samples, white_bkgd=white_bkgd, lindisp=lindisp, mlp_mode=mlp_mode,
-                                         t_stop=t_stop)
+                                         t_stop=t_stop, occupancy=occupancy)
         if writer is not None:
             writer.submit(i, rgb, depth)
         else:

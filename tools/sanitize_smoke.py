@@ -42,6 +42,15 @@ with torch.no_grad():
                 for t_stop in (0.0, 0.5, 2.0):
                     backend.render_rays(many, vol, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=128,
                                         mlp_mode=mode, t_stop=t_stop, tiles_done=torch.zeros(1, dtype=torch.int64, device=dev))
+                # empty-space skipping: the grid build (node samples through the split samples entry, cell reduction,
+                # dilation, packing), then the range pre-pass and the STOP kernels with a range table -- the built grid,
+                # an empty one (every group stored by the pre-pass) and a full one, on the same 1994-ray shape
+                occ = backend.build_occupancy(vol, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), dilate=1)
+                empty = backend.Occupancy(torch.zeros_like(occ.bits), occ.D, occ.Hp, occ.Wp, sc.near_far, sc.pad, False, 1)
+                full = backend.Occupancy(torch.full_like(occ.bits, -1), occ.D, occ.Hp, occ.Wp, sc.near_far, sc.pad, False, 1)
+                for grid in (occ, empty, full):
+                    backend.render_rays(many, vol, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=128,
+                                        mlp_mode=mode, t_stop=0.5, occupancy=grid, white_bkgd=True)
                 # fp16 volume (MVSN_VOLUME_F16): channels-last in place, then planar through mvsn_volume_to_half; both
                 # entries, the sink and the STOP instantiations
                 for vh in (vol.half(), vol.contiguous().half()):
@@ -50,6 +59,9 @@ with torch.no_grad():
                                                             torch.empty(rays.shape[0], device=dev)), sink=sink)
                     backend.render_rays(many, vh, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=128,
                                         mlp_mode=mode, t_stop=0.5, tiles_done=torch.zeros(1, dtype=torch.int64, device=dev))
+                    occ_h = backend.build_occupancy(vh, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad))
+                    backend.render_rays(many, vh, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=128,
+                                        mlp_mode=mode, occupancy=occ_h)
                     xyz_h, _, rd_h, z_h = backend.ray_marcher(rays[:100], N_samples=24)
                     ndc_h = backend.get_ndc_coordinate(d.pose_source["w2cs"][0], d.pose_source["intrinsics"][0], xyz_h,
                                                        torch.tensor([sc.W - 1.0, sc.H - 1.0], device=dev),
