@@ -77,6 +77,12 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// ---- per-warpgroup register budget (executed by every warp of a warpgroup; N a multiple of 8 in [24, 256]) ----
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N)); }
+
 // ---- descriptors -----------------------------------------------------------------------------
 // K-major operand tile stored as 64-element (128-byte) rows, 8-row groups 1024 B apart, 16-byte
 // chunks XOR-swizzled by (row % 8): the SWIZZLE_128B canonical layout.  The tile base must be

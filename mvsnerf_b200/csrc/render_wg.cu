@@ -41,8 +41,22 @@ using namespace hop;
 
 namespace wg {
 constexpr int NWG = 2;                                     // MMA warpgroups (tiles in flight) per CTA
-// fp16: NWG consumers + the producer warpgroup + the loader warp; split: NWG warpgroups + the loader warp
-__host__ __device__ constexpr int threads(bool split) { return split ? NWG * 128 + 32 : (NWG + 1) * 128 + 32; }
+// Three schedules:
+//   fp16 without STOP (rmod): the modulation lives in the consumers' registers.  NWG consumers + the producer
+//        warpgroup + a loader warpgroup (its first warp loads, the other three leave at once); setmaxnreg moves the
+//        producer's and the loader's registers to the consumers.
+//   fp16 with STOP: the modulation in shared memory; NWG consumers + the producer + the loader warp, 128 registers
+//        each.  ptxas does not allocate the STOP consumers beyond the launch budget after a setmaxnreg.inc (they
+//        spill), so they keep the layout without register modulation.
+//   split: NWG warpgroups + the loader warp.
+__host__ __device__ constexpr int threads(bool split, bool rmod) {
+    return split ? NWG * 128 + 32 : rmod ? (NWG + 2) * 128 : (NWG + 1) * 128 + 32;
+}
+__host__ __device__ constexpr int loader_warp(bool split) { return split ? NWG * 4 : (NWG + 1) * 4; }
+// rmod: registers per thread of each role (launched at 65536 / 512 = 128 each).  The consumers hold acc (64) + the
+// next layer's A operand (32) + the modulation (64); the sum over the four warpgroups must fit the 64 K register file.
+constexpr int REGS_CONSUMER = 192, REGS_PRODUCER = 104, REGS_LOADER = 24;
+static_assert((NWG * REGS_CONSUMER + REGS_PRODUCER + REGS_LOADER) * 128 <= 65536, "register file");
 constexpr int ROWS = 64;                                   // samples per tile
 constexpr int NCHUNK = 17;
 // B-operand rows of each chunk (one 64-wide K-block of one layer, consumption order):
@@ -57,9 +71,11 @@ constexpr int BIAS_MOD = 0, BIAS_TRUNK = 128, BIAS_HEAD = 896, BIAS_RGB = 968, B
 __host__ __device__ constexpr int tail_offset(bool split) { return NCHUNK * chunk_stride(split); }
 __host__ __device__ constexpr int image_bytes(bool split) { return tail_offset(split) + BIAS_FLOATS * 4; }
 // shared memory
-//   split: per warpgroup [PE (hi | lo) | MISC (hi | lo) | modulation fp32 | exchange], then the ring, then the biases
-//   fp16:  SLOTS operand-tile slots [PE | MISC], per consumer [modulation fp32 | exchange], then the ring, the biases
-//          = 64 + 2 x 33 + 64 + 4 KB (+ 1 KB alignment) = 199 KB
+//   split:       per warpgroup [PE (hi | lo) | MISC (hi | lo) | modulation fp32 | exchange], the ring (2 stages), the biases
+//   fp16 rmod:   SLOTS operand-tile slots [PE | MISC], per consumer an exchange, the ring (8 stages), the biases
+//                = 64 + 2 x 1 + 128 + 4 KB (+ 1 KB alignment) = 199 KB
+//   fp16 STOP:   SLOTS operand-tile slots, per consumer [modulation fp32 | exchange], the ring (4 stages), the biases
+//                = 64 + 2 x 33 + 64 + 4 KB (+ 1 KB alignment) = 199 KB
 __host__ __device__ constexpr int tile_bytes(bool split) { return split ? 16384 : 8192; }
 __host__ __device__ constexpr int off_misc(bool split) { return tile_bytes(split); }
 constexpr int MOD_BYTES = ROWS * 128 * 4, XCH_BYTES = 1024;
@@ -67,27 +83,36 @@ constexpr int SLOTS = 2 * NWG;                             // fp16: operand-tile
 constexpr int SLOT_BYTES = 2 * 8192;
 __host__ __device__ constexpr int off_mod(bool split) { return 2 * tile_bytes(split); }   // split: inside a warpgroup's region
 __host__ __device__ constexpr int wg_bytes(bool split) { return off_mod(split) + MOD_BYTES + XCH_BYTES; }
-// modulation + exchange of warpgroup w
-__host__ __device__ constexpr int off_state(bool split, int w) {
-    return split ? w * wg_bytes(true) + off_mod(true) : SLOTS * SLOT_BYTES + w * (MOD_BYTES + XCH_BYTES);
+// [modulation |] exchange of warpgroup w (rmod: the exchange alone)
+__host__ __device__ constexpr int off_state(bool split, bool rmod, int w) {
+    return split ? w * wg_bytes(true) + off_mod(true) : SLOTS * SLOT_BYTES + w * ((rmod ? 0 : MOD_BYTES) + XCH_BYTES);
 }
-__host__ __device__ constexpr int nstage(bool split) { return split ? 2 : 4; }
-__host__ __device__ constexpr int off_ring(bool split) { return split ? NWG * wg_bytes(true) : off_state(false, NWG); }
-__host__ __device__ constexpr int off_bias(bool split) { return off_ring(split) + nstage(split) * chunk_stride(split); }
-__host__ __device__ constexpr int smem_bytes(bool split) { return off_bias(split) + BIAS_FLOATS * 4 + 1024; }
-static_assert(smem_bytes(false) <= 227 * 1024 && smem_bytes(true) <= 227 * 1024, "shared memory budget");
-static_assert(wg_bytes(true) % 1024 == 0 && SLOT_BYTES % 1024 == 0 && off_ring(false) % 1024 == 0,
-              "SW128 tiles need 1024-byte alignment");
-// early ray termination (STOP launches only): the pass protocol's state after the biases
+__host__ __device__ constexpr int nstage(bool split, bool rmod) { return split ? 2 : rmod ? 8 : 4; }
+// entries of the static ring barrier arrays: split keeps the four of its original layout, so its kernels (static
+// shared memory offsets included) stay as they were
+__host__ __device__ constexpr int ring_bars(bool split) { return split ? 4 : nstage(false, true); }
+static_assert(nstage(true, false) <= ring_bars(true) && nstage(false, false) <= ring_bars(false), "ring barriers");
+__host__ __device__ constexpr int off_ring(bool split, bool rmod) {
+    return split ? NWG * wg_bytes(true) : off_state(false, rmod, NWG);
+}
+__host__ __device__ constexpr int off_bias(bool split, bool rmod) {
+    return off_ring(split, rmod) + nstage(split, rmod) * chunk_stride(split);
+}
+__host__ __device__ constexpr int smem_bytes(bool split, bool rmod) { return off_bias(split, rmod) + BIAS_FLOATS * 4 + 1024; }
+static_assert(smem_bytes(false, true) <= 227 * 1024 && smem_bytes(true, false) <= 227 * 1024, "shared memory budget");
+static_assert(wg_bytes(true) % 1024 == 0 && SLOT_BYTES % 1024 == 0 && off_ring(false, true) % 1024 == 0 &&
+              off_ring(false, false) % 1024 == 0, "SW128 tiles need 1024-byte alignment");
+// early ray termination (STOP launches only, never rmod): the pass protocol's state after the biases
 constexpr int STOP_BYTES = 128;
-__host__ __device__ constexpr int off_stop(bool split) { return off_bias(split) + BIAS_FLOATS * 4; }
-static_assert(smem_bytes(false) + STOP_BYTES <= 227 * 1024 && smem_bytes(true) + STOP_BYTES <= 227 * 1024,
+__host__ __device__ constexpr int off_stop(bool split) { return off_bias(split, false) + BIAS_FLOATS * 4; }
+static_assert(smem_bytes(false, false) + STOP_BYTES <= 227 * 1024 && smem_bytes(true, false) + STOP_BYTES <= 227 * 1024,
               "shared memory budget");
 }  // namespace wg
 
+template <bool SPLIT>
 struct WgShared {
-    uint64_t full[4];                                      // weight ring
-    uint64_t empty[4];
+    uint64_t full[wg::ring_bars(SPLIT)];                   // weight ring
+    uint64_t empty[wg::ring_bars(SPLIT)];
     uint64_t slot_full[wg::SLOTS];                         // fp16: operand-tile slots
     uint64_t slot_empty[wg::SLOTS];
     Cams cams;
@@ -376,16 +401,17 @@ template <> struct StopRegs<false> { static constexpr bool last = false; };
 // allocation.
 // VT = __half: the encoding volume is stored as fp16 (sc.vol points at halves); only the volume gather changes.
 template <bool FAST, bool SPLIT, bool STOP = false, typename VT = float, typename... Table>
-__global__ void __launch_bounds__(wg::threads(SPLIT), 1)
+__global__ void __launch_bounds__(wg::threads(SPLIT, !SPLIT && !STOP), 1)
 render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict__ wimg, float t_stop,
                  unsigned long long* tiles_done, Table... table) {
     using namespace wg;
-    constexpr int NS = nstage(SPLIT), THREADS = threads(SPLIT);
+    constexpr bool RMOD = !SPLIT && !STOP;               // the modulation in the consumers' registers
+    constexpr int NS = nstage(SPLIT, RMOD), THREADS = threads(SPLIT, RMOD);
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    __shared__ WgShared sh;
+    __shared__ WgShared<SPLIT> sh;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    float* bias = reinterpret_cast<float*>(smem + off_bias(SPLIT));
+    float* bias = reinterpret_cast<float*>(smem + off_bias(SPLIT, RMOD));
 
     load_cams(sc, &sh.cams, tid);
     for (int i = tid; i < BIAS_FLOATS; i += THREADS) bias[i] = __ldg(reinterpret_cast<const float*>(wimg + tail_offset(SPLIT)) + i);
@@ -425,12 +451,16 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
     const int units_total = (G + NWG - 1) / NWG;
     const int my_units = blockIdx.x < units_total ? (units_total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
     const int npass = my_units * NT;
-    const uint32_t ring = smem_u32(smem + off_ring(SPLIT));
+    const uint32_t ring = smem_u32(smem + off_ring(SPLIT, RMOD));
     auto group_of = [&](int pass, int w) { return ((pass / NT) * (int)gridDim.x + (int)blockIdx.x) * NWG + w; };
 
-    if (warp == THREADS / 32 - 1) {
+    // RMOD: each role sets its register budget first thing in its own branch (the loader and the producer give theirs
+    // up to the consumers), so that ptxas allocates every role's code within that role's budget
+    if (SPLIT ? warp == loader_warp(true) : warp >= loader_warp(false)) {
         // =========================== weight loader ===================================================
-        if (elect_one()) {
+        // RMOD: the first warp of the loader warpgroup; the other three leave
+        if constexpr (RMOD) setmaxnreg_dec<REGS_LOADER>();
+        if ((SPLIT || warp == loader_warp(false)) && elect_one()) {
             uint32_t n = 0;
 #pragma unroll 1
             for (int pass = 0; STOP || pass < npass; ++pass) {
@@ -447,7 +477,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                     const uint32_t st = n % NS;
                     if (n >= (uint32_t)NS) mbar_wait(&sh.empty[st], ((n / NS) - 1) & 1);
                     const uint32_t bytes = (uint32_t)chunk_rows(c) * 128;
-                    uint8_t* dst = smem + off_ring(SPLIT) + st * chunk_stride(SPLIT);
+                    uint8_t* dst = smem + off_ring(SPLIT, RMOD) + st * chunk_stride(SPLIT);
                     const uint8_t* src = wimg + (size_t)c * chunk_stride(SPLIT);
                     mbar_arrive_expect_tx(&sh.full[st], SPLIT ? 2 * bytes : bytes);
                     bulk_load(dst, src, bytes, &sh.full[st]);
@@ -461,6 +491,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         if (warp >= NWG * 4) {
             // ======================= producer: front ends of the consumers' tiles, in their order ============
             // consumer w's k-th tile goes to slot 2 w + (k & 1)
+            if constexpr (RMOD) setmaxnreg_dec<REGS_PRODUCER>();
             const int t = tid & 127;
             uint32_t filled[NWG];
 #pragma unroll
@@ -491,13 +522,14 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             }
             return;
         }
+        if constexpr (RMOD) setmaxnreg_inc<REGS_CONSUMER>();
     }
 
     // =========================== MMA warpgroups: one tile at a time ====================================
     const int wgi = warp >> 2, t = tid & 127, w4 = (tid >> 5) & 3, g = lane >> 2, q = lane & 3;
-    uint8_t* state = smem + off_state(SPLIT, wgi);
-    float* modp = reinterpret_cast<float*>(state) + t;                              // [i][128 threads]
-    float* xch = reinterpret_cast<float*>(state + MOD_BYTES);                       // [64 rows][alpha, r, g, b]
+    uint8_t* state = smem + off_state(SPLIT, RMOD, wgi);
+    float* modp = reinterpret_cast<float*>(state) + t;                              // !RMOD: [i][128 threads]
+    float* xch = reinterpret_cast<float*>(state + (RMOD ? 0 : MOD_BYTES));          // [64 rows][alpha, r, g, b]
     const int row_a = w4 * 16 + g, row_b = row_a + 8;
     uint32_t nchunk = 0, ntile = 0;
     auto acquire = [&]() -> uint32_t {
@@ -515,6 +547,13 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
     float cT = 1.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f, c4 = 0.f;   // compositing state of ray t (t < RT)
     float acc[64];
     uint32_t ah[32], al[SPLIT ? 32 : 1];
+    float mod[RMOD ? 64 : 1];                           // RMOD: the modulation of the current tile, accumulator layout
+    auto mod_of = [&](int i) -> float {
+        if constexpr (RMOD) return mod[i];
+        else return modp[i * 128];
+    };
+    // fp16: the bias pair of columns 8 j + 2 q, 8 j + 2 q + 1 (both rows of a thread use it: one 8-byte load)
+    auto bias2 = [&](int base, int j) { return *reinterpret_cast<const float2*>(bias + base + 8 * j + 2 * q); };
     // split: 2^-ew, the scale of the register activation rows row_a / row_b, and the factor that takes the current
     // accumulator rows back to their true values (fp16: all 1)
     const float inv_w = SPLIT ? bias[BIAS_WINV] : 1.f;
@@ -587,15 +626,26 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             pe_u = smem_u32(smem + slot * SLOT_BYTES); misc_u = pe_u + tile_bytes(false);
         }
 
-        // -------------------------- modulation: pts_bias(features), K = 20 -> kept in shared memory ---------
+        // -------------------------- modulation: pts_bias(features), K = 20 -> registers (RMOD) or shared memory
         {
             const uint32_t b = acquire();
             wgmma_fence();
             gemm_ss<128, SPLIT>(acc, misc_u, b, 0, 2, true);
             wgmma_commit(); wgmma_wait<0>(); reg_fence(acc);
             release();
+            if constexpr (!RMOD) {
 #pragma unroll
-            for (int i = 0; i < 64; ++i) modp[i * 128] = fmaf(acc[i], inv_w, bias[BIAS_MOD + col_of(i)]);
+                for (int i = 0; i < 64; ++i) modp[i * 128] = fmaf(acc[i], inv_w, bias[BIAS_MOD + col_of(i)]);
+            } else {
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const float2 bm = bias2(BIAS_MOD, j);
+                    mod[4 * j + 0] = fmaf(acc[4 * j + 0], inv_w, bm.x);
+                    mod[4 * j + 1] = fmaf(acc[4 * j + 1], inv_w, bm.y);
+                    mod[4 * j + 2] = fmaf(acc[4 * j + 2], inv_w, bm.x);
+                    mod[4 * j + 3] = fmaf(acc[4 * j + 3], inv_w, bm.y);
+                }
+            }
         }
         // -------------------------- trunk: six layers, h = relu((W x + b) * mod) -----------------------------
         auto trunk_epilogue = [&](int l) {
@@ -607,11 +657,15 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                 ia = inv_pow2(sa) * inv_w; ib = inv_pow2(sb) * inv_w;
             } else {
 #pragma unroll
-                for (int i = 0; i < 64; i += 2) {
-                    float v0 = (acc[i] + bias[BIAS_TRUNK + l * 128 + col_of(i)]) * modp[i * 128];
-                    float v1 = (acc[i + 1] + bias[BIAS_TRUNK + l * 128 + col_of(i + 1)]) * modp[(i + 1) * 128];
-                    v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
-                    ah[i >> 1] = cvt_h2_sat(v0, v1);
+                for (int j = 0; j < 16; ++j) {
+                    const float2 bt = bias2(BIAS_TRUNK + l * 128, j);
+#pragma unroll
+                    for (int i = 4 * j; i < 4 * j + 4; i += 2) {
+                        float v0 = (acc[i] + bt.x) * mod_of(i);
+                        float v1 = (acc[i + 1] + bt.y) * mod_of(i + 1);
+                        v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
+                        ah[i >> 1] = cvt_h2_sat(v0, v1);
+                    }
                 }
             }
         };
@@ -690,10 +744,14 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                 ia = inv_pow2(sa) * inv_w; ib = inv_pow2(sb) * inv_w;
             } else {
 #pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    const float v0 = fmaxf(h72[i] + bias[BIAS_HEAD + col_of(i)], 0.f);
-                    const float v1 = fmaxf(h72[i + 1] + bias[BIAS_HEAD + col_of(i + 1)], 0.f);
-                    ah[i >> 1] = cvt_h2_sat(v0, v1);
+                for (int j = 0; j < 8; ++j) {
+                    const float2 bh = bias2(BIAS_HEAD, j);
+#pragma unroll
+                    for (int i = 4 * j; i < 4 * j + 4; i += 2) {
+                        const float v0 = fmaxf(h72[i] + bh.x, 0.f);
+                        const float v1 = fmaxf(h72[i + 1] + bh.y, 0.f);
+                        ah[i >> 1] = cvt_h2_sat(v0, v1);
+                    }
                 }
             }
             sig_a = fmaxf(fmaf(h72[32], inv_w, bias[BIAS_HEAD + 64]), 0.f);
@@ -773,29 +831,31 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
 template <typename VT>
 static int set_wg_smem_attributes() {
     using namespace wg;
-    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false)));
-    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, false, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false)));
-    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
-    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, true, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true)));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false, true)));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, false, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false, true)));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true, false)));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, true, false, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true, false)));
     MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, false, true, VT, const int2*>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false) + STOP_BYTES));
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false, false) + STOP_BYTES));
     MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, true, VT, const int2*>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true) + STOP_BYTES));
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true, false) + STOP_BYTES));
     return MVSN_OK;
 }
 
 template <typename VT>
-static void launch_wg_kernel(int grid, int nthreads, int smem, cudaStream_t stream, const SceneDev& sc, const RenderIO& io,
-                             const uint8_t* w, bool fast, bool split, const float* t_stop, unsigned long long* tiles_done,
-                             const int2* ranges) {
+static void launch_wg_kernel(int grid, cudaStream_t stream, const SceneDev& sc, const RenderIO& io, const uint8_t* w, bool fast,
+                             bool split, const float* t_stop, unsigned long long* tiles_done, const int2* ranges) {
     using namespace wg;
     if (t_stop) {                                         // early ray termination: the ray entry only
-        if (split) render_wg_kernel<true, true, true, VT, const int2*><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
-        else       render_wg_kernel<true, false, true, VT, const int2*><<<grid, nthreads, smem + STOP_BYTES, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
+        const int smem = smem_bytes(split, false) + STOP_BYTES, nthreads = threads(split, false);
+        if (split) render_wg_kernel<true, true, true, VT, const int2*><<<grid, nthreads, smem, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
+        else       render_wg_kernel<true, false, true, VT, const int2*><<<grid, nthreads, smem, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
     } else if (split) {
+        const int smem = smem_bytes(true, false), nthreads = threads(true, false);
         if (fast) render_wg_kernel<true, true, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
         else      render_wg_kernel<false, true, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
     } else {
+        const int smem = smem_bytes(false, true), nthreads = threads(false, true);
         if (fast) render_wg_kernel<true, false, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
         else      render_wg_kernel<false, false, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);
     }
@@ -824,7 +884,6 @@ int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool 
     const int grid = units < sm_count() ? units : sm_count();
     if (grid <= 0) return MVSN_OK;
     const uint8_t* w = static_cast<const uint8_t*>(wimg);
-    const int smem = smem_bytes(split), nthreads = threads(split);
     if (occ_bits) {                                       // empty-space skipping: the range pre-pass at this launch's rt
         if (!t_stop || !ranges) { set_error("launch_render_wg: an occupancy grid needs t_stop and a range table"); return MVSN_EBADSHAPE; }
         const int rc = launch_occupancy_ranges(sc, io, split, occ_bits, ranges, stream);
@@ -832,8 +891,8 @@ int launch_render_wg(const SceneDev& sc, const RenderIO& io_in, bool fast, bool 
     } else {
         ranges = nullptr;
     }
-    if (half_vol) launch_wg_kernel<__half>(grid, nthreads, smem, stream, sc, io, w, fast, split, t_stop, tiles_done, ranges);
-    else          launch_wg_kernel<float>(grid, nthreads, smem, stream, sc, io, w, fast, split, t_stop, tiles_done, ranges);
+    if (half_vol) launch_wg_kernel<__half>(grid, stream, sc, io, w, fast, split, t_stop, tiles_done, ranges);
+    else          launch_wg_kernel<float>(grid, stream, sc, io, w, fast, split, t_stop, tiles_done, ranges);
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;
 }
