@@ -15,7 +15,8 @@
 //                        overlaps the GEMMs and epilogues of the others.
 //   last warp            weight loader: one thread streams the weight image, one K-block of one layer at a
 //                        time, L2 -> a shared-memory ring with 1-D bulk async copies (mbarrier complete_tx);
-//                        every consumer consumes the same chunk sequence.
+//                        every consumer consumes the same chunk sequence.  fp16 without STOP: half of the image
+//                        (RES_MASK) is copied once and stays resident; only the other chunks are streamed.
 // Split mode (hi | lo operands, twice the operand bytes) does not fit the slot ring in shared memory, so there
 // every warpgroup runs its own front end before its GEMMs (NWG + 1 roles, no producer).
 // feature_linear has no non-linearity before views_linears[0] (models.py:213-218): the two are folded at pack
@@ -70,10 +71,27 @@ constexpr int BIAS_MOD = 0, BIAS_TRUNK = 128, BIAS_HEAD = 896, BIAS_RGB = 968, B
               BIAS_FLOATS = 1024;
 __host__ __device__ constexpr int tail_offset(bool split) { return NCHUNK * chunk_stride(split); }
 __host__ __device__ constexpr int image_bytes(bool split) { return tail_offset(split) + BIAS_FLOATS * 4; }
+// rmod: the chunks that stay resident in shared memory for the whole kernel (copied once per CTA): the modulation,
+// layer 0, the folded head, rgb and three trunk chunks spread between the streamed ones.  The other eight chunks
+// (128 KB per pass instead of 236) are streamed through the ring.
+constexpr uint32_t RES_MASK = 0x3u | (1u << 4) | (1u << 7) | (1u << 10) | 0x1E000u;
+__host__ __device__ constexpr bool resident(int c) { return (RES_MASK >> c) & 1u; }
+static_assert((RES_MASK >> 13) == 0xFu, "the folded head and rgb are resident");
+__host__ __device__ constexpr uint32_t popc32(uint32_t x) {
+    x = x - ((x >> 1) & 0x55555555u);
+    x = (x & 0x33333333u) + ((x >> 2) & 0x33333333u);
+    return (((x + (x >> 4)) & 0x0F0F0F0Fu) * 0x01010101u) >> 24;
+}
+// byte offset of resident chunk c in the resident region: the resident chunks in order, the 128-row ones (16 KB) before
+// the head's 72-row ones (9 KB) -- multiples of the 1024 that SW128 tiles need
+__host__ __device__ constexpr uint32_t res_offset(int c) {
+    return 16384u * popc32(RES_MASK & ((1u << (c < 13 ? c : 13)) - 1u)) + 9216u * (c > 13 ? c - 13 : 0);
+}
+constexpr int NSTREAM = NCHUNK - (int)popc32(RES_MASK), RES_BYTES = (int)res_offset(NCHUNK - 1) + 1024;
 // shared memory
 //   split:       per warpgroup [PE (hi | lo) | MISC (hi | lo) | modulation fp32 | exchange], the ring (2 stages), the biases
-//   fp16 rmod:   SLOTS operand-tile slots [PE | MISC], per consumer an exchange, the ring (8 stages), the biases
-//                = 64 + 2 x 1 + 128 + 4 KB (+ 1 KB alignment) = 199 KB
+//   fp16 rmod:   SLOTS operand-tile slots [PE | MISC], per consumer an exchange, the ring (2 stages), the resident
+//                chunks, the biases = 64 + 2 x 1 + 32 + 108 + 4 KB (+ 1 KB alignment) = 211 KB
 //   fp16 STOP:   SLOTS operand-tile slots, per consumer [modulation fp32 | exchange], the ring (4 stages), the biases
 //                = 64 + 2 x 33 + 64 + 4 KB (+ 1 KB alignment) = 199 KB
 __host__ __device__ constexpr int tile_bytes(bool split) { return split ? 16384 : 8192; }
@@ -87,21 +105,28 @@ __host__ __device__ constexpr int wg_bytes(bool split) { return off_mod(split) +
 __host__ __device__ constexpr int off_state(bool split, bool rmod, int w) {
     return split ? w * wg_bytes(true) + off_mod(true) : SLOTS * SLOT_BYTES + w * ((rmod ? 0 : MOD_BYTES) + XCH_BYTES);
 }
-__host__ __device__ constexpr int nstage(bool split, bool rmod) { return split ? 2 : rmod ? 8 : 4; }
-// entries of the static ring barrier arrays: split keeps the four of its original layout, so its kernels (static
-// shared memory offsets included) stay as they were
-__host__ __device__ constexpr int ring_bars(bool split) { return split ? 4 : nstage(false, true); }
-static_assert(nstage(true, false) <= ring_bars(true) && nstage(false, false) <= ring_bars(false), "ring barriers");
+__host__ __device__ constexpr int nstage(bool split, bool rmod) { return split ? 2 : rmod ? 2 : 4; }
+// entries of the static ring barrier arrays: split keeps the four and fp16 the eight of their earlier layouts, so the
+// split and STOP kernels (static shared memory offsets included) stay as they were
+__host__ __device__ constexpr int ring_bars(bool split) { return split ? 4 : 8; }
+static_assert(nstage(true, false) <= ring_bars(true) && nstage(false, false) <= ring_bars(false) &&
+              nstage(false, true) <= ring_bars(false), "ring barriers");
+// rmod: a consumer takes the streamed stages of a whole layer before its first wgmma (trunk layers 1-5: chunks 2-3,
+// 4-5, 6-7, 8-9, 10-12), so the ring must hold them
+static_assert(popc32(~RES_MASK & 0xCu) <= nstage(false, true) && popc32(~RES_MASK & 0x30u) <= nstage(false, true) &&
+              popc32(~RES_MASK & 0xC0u) <= nstage(false, true) && popc32(~RES_MASK & 0x300u) <= nstage(false, true) &&
+              popc32(~RES_MASK & 0x1C00u) <= nstage(false, true), "ring depth");
 __host__ __device__ constexpr int off_ring(bool split, bool rmod) {
     return split ? NWG * wg_bytes(true) : off_state(false, rmod, NWG);
 }
+__host__ __device__ constexpr int off_res() { return off_ring(false, true) + nstage(false, true) * HALF_STRIDE; }   // rmod
 __host__ __device__ constexpr int off_bias(bool split, bool rmod) {
-    return off_ring(split, rmod) + nstage(split, rmod) * chunk_stride(split);
+    return off_ring(split, rmod) + nstage(split, rmod) * chunk_stride(split) + (rmod ? RES_BYTES : 0);
 }
 __host__ __device__ constexpr int smem_bytes(bool split, bool rmod) { return off_bias(split, rmod) + BIAS_FLOATS * 4 + 1024; }
-static_assert(smem_bytes(false, true) <= 227 * 1024 && smem_bytes(true, false) <= 227 * 1024, "shared memory budget");
+static_assert(smem_bytes(true, false) <= 227 * 1024, "shared memory budget");
 static_assert(wg_bytes(true) % 1024 == 0 && SLOT_BYTES % 1024 == 0 && off_ring(false, true) % 1024 == 0 &&
-              off_ring(false, false) % 1024 == 0, "SW128 tiles need 1024-byte alignment");
+              off_ring(false, false) % 1024 == 0 && off_res() % 1024 == 0, "SW128 tiles need 1024-byte alignment");
 // early ray termination (STOP launches only, never rmod): the pass protocol's state after the biases
 constexpr int STOP_BYTES = 128;
 __host__ __device__ constexpr int off_stop(bool split) { return off_bias(split, false) + BIAS_FLOATS * 4; }
@@ -117,6 +142,11 @@ struct WgShared {
     uint64_t slot_empty[wg::SLOTS];
     Cams cams;
 };
+// rmod: one more barrier, for the one-shot copy of the resident chunks (appended, so the other kernels' layout stays)
+struct WgSharedRes : WgShared<false> {
+    uint64_t resident;
+};
+static_assert(wg::smem_bytes(false, true) + sizeof(WgSharedRes) <= 227 * 1024, "shared memory budget");
 
 // STOP: every consumer publishes, at the start of pass p, what it computes in pass p + 2 (its plan); dec[(p + 2) & 3]
 // completes when all consumers have (the plans of passes 0 and 1 are set up before the roles split).  The loader, the
@@ -409,7 +439,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
     constexpr int NS = nstage(SPLIT, RMOD), THREADS = threads(SPLIT, RMOD);
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    __shared__ WgShared<SPLIT> sh;
+    __shared__ std::conditional_t<RMOD, WgSharedRes, WgShared<SPLIT>> sh;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     float* bias = reinterpret_cast<float*>(smem + off_bias(SPLIT, RMOD));
 
@@ -419,6 +449,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         for (int i = 0; i < NS; ++i) { mbar_init(&sh.full[i], 1); mbar_init(&sh.empty[i], NWG * 4); }
         if (!SPLIT)
             for (int i = 0; i < SLOTS; ++i) { mbar_init(&sh.slot_full[i], 128); mbar_init(&sh.slot_empty[i], 4); }
+        if constexpr (RMOD) mbar_init(&sh.resident, 1);
         if constexpr (STOP) {
             WgStop* ss = stop_state(smem, SPLIT);
             const int G0 = (io.N + io.rays_per_tile - 1) / io.rays_per_tile;
@@ -462,26 +493,47 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         if constexpr (RMOD) setmaxnreg_dec<REGS_LOADER>();
         if ((SPLIT || warp == loader_warp(false)) && elect_one()) {
             uint32_t n = 0;
-#pragma unroll 1
-            for (int pass = 0; STOP || pass < npass; ++pass) {
-                if constexpr (STOP) {                    // one pass of NCHUNK chunks while any consumer has work
-                    WgStop* ss = stop_state(smem, SPLIT);
-                    stop_wait(ss, pass);
-                    bool any = false;
+            if constexpr (RMOD) {                        // the resident chunks once, then only the streamed ones
+                mbar_arrive_expect_tx(&sh.resident, RES_BYTES);
 #pragma unroll
-                    for (int w = 0; w < NWG; ++w) any |= stop_busy(ss, pass, w);
-                    if (!any) break;
-                }
+                for (int c = 0; c < NCHUNK; ++c)
+                    if (resident(c))
+                        bulk_load(smem + off_res() + res_offset(c), wimg + (size_t)c * HALF_STRIDE, chunk_rows(c) * 128, &sh.resident);
 #pragma unroll 1
-                for (int c = 0; c < NCHUNK; ++c, ++n) {
-                    const uint32_t st = n % NS;
-                    if (n >= (uint32_t)NS) mbar_wait(&sh.empty[st], ((n / NS) - 1) & 1);
-                    const uint32_t bytes = (uint32_t)chunk_rows(c) * 128;
-                    uint8_t* dst = smem + off_ring(SPLIT, RMOD) + st * chunk_stride(SPLIT);
-                    const uint8_t* src = wimg + (size_t)c * chunk_stride(SPLIT);
-                    mbar_arrive_expect_tx(&sh.full[st], SPLIT ? 2 * bytes : bytes);
-                    bulk_load(dst, src, bytes, &sh.full[st]);
-                    if (SPLIT) bulk_load(dst + HALF_STRIDE, src + HALF_STRIDE, bytes, &sh.full[st]);
+                for (int pass = 0; pass < npass; ++pass) {
+#pragma unroll 1
+                    for (int c = 0; c < NCHUNK; ++c) {
+                        if (resident(c)) continue;
+                        const uint32_t st = n % NS;
+                        if (n >= (uint32_t)NS) mbar_wait(&sh.empty[st], ((n / NS) - 1) & 1);
+                        const uint32_t bytes = (uint32_t)chunk_rows(c) * 128;
+                        mbar_arrive_expect_tx(&sh.full[st], bytes);
+                        bulk_load(smem + off_ring(false, true) + st * HALF_STRIDE, wimg + (size_t)c * HALF_STRIDE, bytes, &sh.full[st]);
+                        ++n;
+                    }
+                }
+            } else {
+#pragma unroll 1
+                for (int pass = 0; STOP || pass < npass; ++pass) {
+                    if constexpr (STOP) {                    // one pass of NCHUNK chunks while any consumer has work
+                        WgStop* ss = stop_state(smem, SPLIT);
+                        stop_wait(ss, pass);
+                        bool any = false;
+#pragma unroll
+                        for (int w = 0; w < NWG; ++w) any |= stop_busy(ss, pass, w);
+                        if (!any) break;
+                    }
+#pragma unroll 1
+                    for (int c = 0; c < NCHUNK; ++c, ++n) {
+                        const uint32_t st = n % NS;
+                        if (n >= (uint32_t)NS) mbar_wait(&sh.empty[st], ((n / NS) - 1) & 1);
+                        const uint32_t bytes = (uint32_t)chunk_rows(c) * 128;
+                        uint8_t* dst = smem + off_ring(SPLIT, RMOD) + st * chunk_stride(SPLIT);
+                        const uint8_t* src = wimg + (size_t)c * chunk_stride(SPLIT);
+                        mbar_arrive_expect_tx(&sh.full[st], SPLIT ? 2 * bytes : bytes);
+                        bulk_load(dst, src, bytes, &sh.full[st]);
+                        if (SPLIT) bulk_load(dst + HALF_STRIDE, src + HALF_STRIDE, bytes, &sh.full[st]);
+                    }
                 }
             }
         }
@@ -522,7 +574,10 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             }
             return;
         }
-        if constexpr (RMOD) setmaxnreg_inc<REGS_CONSUMER>();
+        if constexpr (RMOD) {
+            setmaxnreg_inc<REGS_CONSUMER>();
+            mbar_wait(&sh.resident, 0);                  // the resident chunks have landed
+        }
     }
 
     // =========================== MMA warpgroups: one tile at a time ====================================
@@ -532,15 +587,50 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
     float* xch = reinterpret_cast<float*>(state + (RMOD ? 0 : MOD_BYTES));          // [64 rows][alpha, r, g, b]
     const int row_a = w4 * 16 + g, row_b = row_a + 8;
     uint32_t nchunk = 0, ntile = 0;
-    auto acquire = [&]() -> uint32_t {
-        const uint32_t st = nchunk % NS;
-        mbar_wait(&sh.full[st], (nchunk / NS) & 1);
+    // the k-th streamed chunk after the oldest one not yet released (k > 0: RMOD only)
+    auto acquire = [&](uint32_t k = 0) -> uint32_t {
+        const uint32_t st = (nchunk + k) % NS;
+        mbar_wait(&sh.full[st], ((nchunk + k) / NS) & 1);
         return ring + st * chunk_stride(SPLIT);
     };
     auto release = [&]() {
         __syncwarp();
         if (lane == 0) mbar_arrive(&sh.empty[nchunk % NS]);
         ++nchunk;
+    };
+    // A layer of chunks c0 .. c0 + n - 1: layer_begin(c0, b[n]); per chunk i: chunk_begin(b[i]), wgmma_fence(), its
+    // wgmmas, chunk_end(c0 + i, i == 0, d); then layer_end(c0 + n - 1, d).  Without RMOD every chunk is streamed,
+    // acquired and drained on its own.  RMOD: layer_begin takes the B operands of the whole layer before its first wgmma
+    // -- a resident chunk's is a constant address, a streamed one's waits for its stage -- and the layer's wgmma groups
+    // stay in flight until one wait before its epilogue.  A streamed stage is released once the group that read it has
+    // retired: wgmma_wait<1> after the layer's next group, or the layer's wait.
+    const uint32_t res = ring + (off_res() - off_ring(false, true));
+    auto layer_begin = [&](int c0, auto& b) {
+        if constexpr (RMOD) {
+            uint32_t k = 0;                              // the layer's streamed chunks taken so far
+#pragma unroll
+            for (int i = 0; i < (int)(sizeof(b) / sizeof(b[0])); ++i)
+                b[i] = resident(c0 + i) ? res + res_offset(c0 + i) : acquire(k++);
+        }
+    };
+    auto chunk_begin = [&](uint32_t b) -> uint32_t {
+        if constexpr (RMOD) return b;
+        else return acquire();
+    };
+    auto chunk_end = [&](int c, bool first, auto& d) {
+        wgmma_commit();
+        if constexpr (!RMOD) {
+            wgmma_wait<0>(); reg_fence(d);
+            release();
+        } else if (!first && !resident(c - 1)) {
+            wgmma_wait<1>(); release();
+        }
+    };
+    auto layer_end = [&](int c, auto& d) {
+        if constexpr (RMOD) {
+            wgmma_wait<0>(); reg_fence(d);
+            if (!resident(c)) release();
+        }
     };
     auto col_of = [&](int i) { return 8 * (i >> 2) + 2 * q + (i & 1); };
 
@@ -604,7 +694,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         } else {
             if (grp >= G) {                              // idle in the final passes: keep the weight ring moving
 #pragma unroll 1
-                for (int c = 0; c < NCHUNK; ++c) { acquire(); release(); }
+                for (int c = 0; c < (RMOD ? NSTREAM : NCHUNK); ++c) { acquire(); release(); }
                 continue;
             }
         }
@@ -628,11 +718,12 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
 
         // -------------------------- modulation: pts_bias(features), K = 20 -> registers (RMOD) or shared memory
         {
-            const uint32_t b = acquire();
+            uint32_t bl[1];
+            layer_begin(0, bl);
+            const uint32_t b = chunk_begin(bl[0]);
             wgmma_fence();
             gemm_ss<128, SPLIT>(acc, misc_u, b, 0, 2, true);
-            wgmma_commit(); wgmma_wait<0>(); reg_fence(acc);
-            release();
+            chunk_end(0, true, acc); layer_end(0, acc);
             if constexpr (!RMOD) {
 #pragma unroll
                 for (int i = 0; i < 64; ++i) modp[i * 128] = fmaf(acc[i], inv_w, bias[BIAS_MOD + col_of(i)]);
@@ -670,57 +761,62 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
             }
         };
         {   // layer 0: A = encoding (63 columns)
-            const uint32_t b = acquire();
+            uint32_t bl[1];
+            layer_begin(1, bl);
+            const uint32_t b = chunk_begin(bl[0]);
             wgmma_fence();
             gemm_ss<128, SPLIT>(acc, pe_u, b, 0, 4, true);
-            wgmma_commit(); wgmma_wait<0>(); reg_fence(acc);
-            release();
+            chunk_end(1, true, acc); layer_end(1, acc);
             ia = ib = inv_w;
             trunk_epilogue(0);
         }
 #pragma unroll 1
         for (int l = 1; l <= 4; ++l) {
+            uint32_t bl[2];
+            layer_begin(2 * l, bl);
 #pragma unroll
             for (int kb = 0; kb < 2; ++kb) {
-                const uint32_t b = acquire();
+                const uint32_t b = chunk_begin(bl[kb]);
                 wgmma_fence();
                 gemm_rs<128, SPLIT>(acc, ah, al, b, kb, kb == 0);
-                wgmma_commit(); wgmma_wait<0>(); reg_fence(acc);
-                release();
+                chunk_end(2 * l + kb, kb == 0, acc);
             }
+            layer_end(2 * l + 1, acc);
             trunk_epilogue(l);
         }
         {   // layer 5: A = [encoding | h] (skip connection after layer 4)
-            uint32_t b = acquire();
+            uint32_t bl[3];
+            layer_begin(10, bl);
+            uint32_t b = chunk_begin(bl[0]);
             wgmma_fence();
             gemm_ss<128, SPLIT>(acc, pe_u, b, 0, 4, true);
-            wgmma_commit(); wgmma_wait<0>(); reg_fence(acc);
-            release();
+            chunk_end(10, true, acc);
             if constexpr (SPLIT) {                     // to the scale of the register rows (exact: powers of two)
 #pragma unroll
                 for (int i = 0; i < 64; ++i) acc[i] *= (i & 2) ? sb : sa;
             }
 #pragma unroll
             for (int kb = 0; kb < 2; ++kb) {
-                b = acquire();
+                b = chunk_begin(bl[1 + kb]);
                 wgmma_fence();
                 gemm_rs<128, SPLIT>(acc, ah, al, b, kb, false);
-                wgmma_commit(); wgmma_wait<0>(); reg_fence(acc);
-                release();
+                chunk_end(11 + kb, false, acc);
             }
+            layer_end(12, acc);
             trunk_epilogue(5);
         }
         // -------------------------- folded head: views layer (64) + alpha (col 64) ---------------------------
         float sig_a = 0.f, sig_b = 0.f;
         {
             float h72[36];
+            uint32_t bl[3];
+            layer_begin(13, bl);
 #pragma unroll
             for (int kb = 0; kb < 2; ++kb) {
-                const uint32_t b = acquire();
+                const uint32_t b = chunk_begin(bl[kb]);
                 wgmma_fence();
                 gemm_rs<72, SPLIT>(h72, ah, al, b, kb, kb == 0);
-                wgmma_commit(); wgmma_wait<0>(); reg_fence(h72);
-                release();
+                chunk_end(13 + kb, kb == 0, h72);
             }
             if constexpr (SPLIT) {                     // back to the front-end scale of the view-direction columns
                 const float ra = inv_pow2(sa), rb = inv_pow2(sb);
@@ -728,11 +824,10 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
                 for (int i = 0; i < 36; ++i) h72[i] *= (i & 2) ? rb : ra;
             }
             {   // view direction: MISC K-step 2 (cols 32..47)
-                const uint32_t b = acquire();
+                const uint32_t b = chunk_begin(bl[2]);
                 wgmma_fence();
                 gemm_ss<72, SPLIT>(h72, misc_u, b, 2, 1, false);
-                wgmma_commit(); wgmma_wait<0>(); reg_fence(h72);
-                release();
+                chunk_end(15, false, h72); layer_end(15, h72);
                 if constexpr (!SPLIT) {                // the last read of the operand tiles: free the slot
                     if (lane == 0) mbar_arrive(&sh.slot_empty[slot]);
                 }
@@ -760,11 +855,12 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
         // -------------------------- rgb (N = 8, 3 used) -------------------------------------------------------
         {
             float r8[4];
-            const uint32_t b = acquire();
+            uint32_t bl[1];
+            layer_begin(16, bl);
+            const uint32_t b = chunk_begin(bl[0]);
             wgmma_fence();
             gemm_rs<8, SPLIT>(r8, ah, al, b, 0, true);
-            wgmma_commit(); wgmma_wait<0>(); reg_fence(r8);
-            release();
+            chunk_end(16, true, r8); layer_end(16, r8);
             auto sigm = [&](float x) { return SPLIT ? __fdiv_rn(1.f, 1.f + expf(-x)) : __fdividef(1.f, 1.f + __expf(-x)); };
             if (q == 0) {
                 xch[row_a * 4 + 0] = 1.f - (SPLIT ? expf(-sig_a) : __expf(-sig_a));
