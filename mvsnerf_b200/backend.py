@@ -951,12 +951,28 @@ def ray_marcher(rays, N_samples=64, lindisp=False, perturb=0):
     return xyz, rays_o, rays_d, z_vals
 
 
+def _matmul3(p, m):
+    """p [M,3] @ m[3,3]^T as an FMA-capable BLAS computes it for fp32: row r = fma(p2, m[r,2], fma(p1, m[r,1], p0 m[r,0])),
+    each fma formed in fp64 (where the product of two floats is exact) and rounded to fp32.  torch.matmul's rounding of
+    these 3-term dot products depends on the CPU's BLAS code path (without FMA it rounds every product); this order is
+    the one of the reference run on AVX2 / AVX-512 hosts and of the kernels' ndc_of_point, on any host.  Other dtypes:
+    torch.matmul."""
+    if p.dtype != torch.float32 or m.dtype != torch.float32:
+        return torch.matmul(p, m.t())
+    pd, md = p.double(), m.double()
+    out = p[:, :1] * m[:, 0].reshape(1, 3)
+    for k in (1, 2):
+        out = (pd[:, k:k + 1] * md[:, k].reshape(1, 3) + out.double()).float()
+    return out
+
+
 def get_ndc_coordinate(w2c_ref, intrinsic_ref, point_samples, inv_scale, near=2, far=6, pad=0, lindisp=False):
-    """utils.py:112-146 (projection branch): world points [N,S,3] -> volume coordinates in [0,1]."""
+    """utils.py:112-146 (projection branch): world points [N,S,3] -> volume coordinates in [0,1].  The two 3x3 products
+    are rounded as _matmul3 states, the same on every host."""
     n, s = point_samples.shape[:2]
     p = point_samples.reshape(-1, 3)
-    p = torch.matmul(p, w2c_ref[:3, :3].t()) + w2c_ref[:3, 3:].reshape(1, 3)
-    q = p @ intrinsic_ref.t()
+    p = _matmul3(p, w2c_ref[:3, :3]) + w2c_ref[:3, 3:].reshape(1, 3)
+    q = _matmul3(p, intrinsic_ref)
     q[:, :2] = (q[:, :2] / q[:, -1:] + 0.0) / inv_scale.reshape(1, 2)
     if not lindisp:
         q[:, 2] = (q[:, 2] - near) / (far - near)
