@@ -43,6 +43,17 @@ extern "C" {
 #define MVSN_MLP_TC_PAIR     3  /* same kernel and image as TC_HALF (the bench headline): weights     */
                                 /* streamed, activations in registers, views/feature layers folded  */
                                 /* (TC modes take any N_samples; rays are tiled up to 32 at a time)    */
+/* grad_mode of the rays fine-tuning entries only (mvsn_render_backward_rays / _rays_stop and their workspace sizes):
+ * MVSN_MLP_TC_HALF's backward plus the forward recompute's MLP on wgmma.  GEMMs with N >= 64 (pts_bias, layers 0-5,
+ * feature_linear, the 128 feature columns of views_linears.0) take fp16 operands with fp32 accumulation; hidden
+ * activations carry an exact power-of-two scale per sample row (row maximum in [2^14, 2^15)), the encoding and the 20
+ * features are unscaled, weights are rounded unscaled, conversions saturate; layer 5's encoding and h parts are
+ * combined by an exact power-of-two rescale.  alpha_linear, rgb_linear and the view-direction columns stay FFMA on
+ * operands rounded to fp16's significand; biases, modulation, activations, compositing and the front end stay fp32.
+ * A row's result depends on that row only: a ray's rgb, depth and loss term do not depend on the other rays of the
+ * batch, and the early-termination recompute repeats the first bit for bit.  rgb is within the 5e-3 tier of
+ * MVSN_MLP_FP32. */
+#define MVSN_GRAD_TC_FULL    4
 #define MVSN_VOLUME_F16      0x100 /* flag OR-ed into mvsn_render_scene.mlp_mode with a TC mode: volume_dhwc points at an */
                                 /* fp16 [D,Hp,Wp,8] image (16-byte aligned).  Each value is widened exactly to fp32, so a  */
                                 /* render is bit-identical to one from the fp32 volume vol.half().float(); the storage     */
@@ -257,7 +268,8 @@ int mvsn_render_backward_tc(const mvsn_render_scene* scene, const float* const* 
  * from the largest |gradient| (contributions below ~max|g| * N * S * 2^-62 round to zero) and ACCUMULATED into
  * grad_volume_dhwc, and loss_out is ACCUMULATED with the per-ray terms summed in a fixed order.  rgb_out / depth_out
  * and the MLP gradients are the same as the non-deterministic entry's.  A non-finite gradient makes the volume
- * entries it touches NaN / inf as the atomics would.  Any other grad_mode: MVSN_EUNSUPPORTED, before any CUDA call.
+ * entries it touches NaN / inf as the atomics would.  Any other grad_mode (MVSN_GRAD_TC_FULL included: rays entries
+ * only): MVSN_EUNSUPPORTED, before any CUDA call.
  * Workspace: mvsn_render_backward_deterministic_workspace_bytes(N, S, D, Hp, Wp, grad_mode), 16-byte aligned, with the
  * scene's volume dims (it holds a [D,Hp,Wp,8] int64 accumulator, zeroed by every call); D = Hp = Wp = 0 sizes it for a
  * frozen volume (grad_volume_dhwc = NULL).  0 for an unknown grad_mode or shape. */
@@ -274,7 +286,8 @@ int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const flo
  * mvsn_render_rays'): sample s of a ray lies at lower + (upper - lower) * jitter, between the midpoints of the
  * neighbouring unjittered depths (data/ray_utils.py:184-191), each operation rounded as fp32 element-wise ops round it.
  * grad_mode MVSN_MLP_FP32 or MVSN_MLP_TC_HALF selects the arithmetic of the GEMMs as mvsn_render_backward /
- * mvsn_render_backward_tc do; deterministic != 0 sums the volume gradient and the loss as
+ * mvsn_render_backward_tc do, MVSN_GRAD_TC_FULL also moves the forward recompute to tensor cores (see its define;
+ * rgb_out / depth_out / the loss are then this mode's forward); deterministic != 0 sums the volume gradient and the loss as
  * mvsn_render_backward_deterministic does.  g, grad_mlp and grad_volume_dhwc as mvsn_render_backward; rgb_out /
  * depth_out receive the forward of the marched samples (with jitter = NULL: rgb bit-identical to mvsn_render_rays with
  * the MVSN_MLP_FP32 image).  N_samples <= 128.  Argument errors are returned before any CUDA call: an unknown grad_mode
@@ -288,13 +301,13 @@ int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const
                               int deterministic, const mvsn_render_grads* g, float* const* grad_mlp,
                               float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream);
 /* mvsn_render_backward_rays_stop: mvsn_render_backward_rays with early ray termination.  For each ray, with alpha_j
- * from the fp32 recompute, T_0 = 1 and T_{j+1} = T_j ((1 - alpha_j) + 1e-10) (the kernel's fp32 order), sample j is
+ * from this mode's recompute, T_0 = 1 and T_{j+1} = T_j ((1 - alpha_j) + 1e-10) (the kernel's fp32 order), sample j is
  * live iff T_j >= t_stop; the live samples are a prefix of length L (L >= 1).  The step renders, forms the loss of and
  * exactly differentiates the truncated render sum_{j<L} w_j c_j (depth and white_bkgd likewise); dead samples get no
  * gradient and no volume scatter.  Against the full render, per channel -t_stop < rgb - rgb_full <= 0 (white_bkgd:
  * 0 <= rgb - rgb_full < t_stop) and 0 <= depth_full - depth < t_stop * far, up to a few ulps.  t_stop = 0 keeps every
- * sample: every output is bit-identical to mvsn_render_backward_rays.  With MVSN_MLP_FP32 a ray's rgb, depth and loss
- * term do not depend on the other rays of the batch; the MLP gradients may differ from a differently packed batch in
+ * sample: every output is bit-identical to mvsn_render_backward_rays.  With MVSN_MLP_FP32 or MVSN_GRAD_TC_FULL a ray's rgb, depth
+ * and loss term do not depend on the other rays of the batch; the MLP gradients may differ from a differently packed batch in
  * summation order only.  deterministic != 0: every output is a deterministic function of the inputs.
  * live_samples [N] int32 (device, 4-byte aligned, may be NULL): each ray's L.  tiles_done (device, 8-byte aligned, may
  * be NULL): unsigned long long[3] += the 128-row tiles back-propagated immediately, deferred, and packed from deferred

@@ -632,8 +632,14 @@ BACKWARD_IMPL = "kernel"
 _bwd_workspace = {}
 
 
-def _check_grad_mode(grad_mode):
-    if grad_mode not in (_lib.MLP_FP32, _lib.MLP_TC_HALF):
+def _check_grad_mode(grad_mode, rays=False):
+    """`rays`: the entry marches its samples from rays (render_backward_rays, FineTuner.step_rays), the only ones that
+    take GRAD_TC_FULL."""
+    if grad_mode == _lib.GRAD_TC_FULL and not rays:
+        raise RuntimeError("grad_mode GRAD_TC_FULL (the forward recompute on tensor cores too) is taken by "
+                           "FineTuner.step_rays and render_backward_rays only; the samples entries (FineTuner.step, "
+                           "render_backward, rendering under autograd) run MLP_FP32 or MLP_TC_HALF")
+    if grad_mode not in (_lib.MLP_FP32, _lib.MLP_TC_HALF, _lib.GRAD_TC_FULL):
         raise RuntimeError(f"grad_mode {grad_mode!r}: the backward's GEMMs run in MLP_FP32 (FFMA) or MLP_TC_HALF "
                            "(wgmma, fp16 operands with per-tile power-of-two scales, fp32 accumulation)")
 
@@ -772,8 +778,12 @@ def render_backward_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_
     bit-identical to t_stop=None).  Per-sample cotangents (`grads` 'weights', 'alpha', 'input_feat') are rejected with
     it.  `live_samples`: an optional CUDA int32 tensor [N] that receives each ray's number of kept samples;
     `tiles_done`: an optional CUDA int64 tensor [3] the counts of tiles back-propagated immediately, deferred and packed
-    are added to."""
-    _check_grad_mode(grad_mode)
+    are added to.
+
+    grad_mode=GRAD_TC_FULL: MLP_TC_HALF's backward, and the forward recompute's MLP on tensor cores too (fp16 operands,
+    a power-of-two scale per sample row, fp32 accumulation; see MVSN_GRAD_TC_FULL in include/mvsnerf_b200.h).  rgb,
+    depth and the loss are then that recompute's, within the 5e-3 tier of MLP_FP32."""
+    _check_grad_mode(grad_mode, rays=True)
     if t_stop is not None:
         t_stop = float(t_stop)
         if not 0.0 <= t_stop <= 1.0:
@@ -839,14 +849,15 @@ class FineTuner:
 
     The parameters stay the caller's nn.Parameters (updated in place, version counters bumped), so checkpoints, the
     render entry points and scene_io see them as after a torch.optim.Adam step with the same hyper-parameters.
-    grad_mode=MLP_TC_HALF runs the backward's dgrad / wgrad GEMMs on tensor cores (see render_backward).  Under
+    grad_mode=MLP_TC_HALF runs the backward's dgrad / wgrad GEMMs on tensor cores (see render_backward);
+    grad_mode=GRAD_TC_FULL (step_rays only) also its forward recompute (see render_backward_rays).  Under
     torch.use_deterministic_algorithms(True) every step is bit-reproducible: two runs from the same start on the same
     batches end with identical parameters, volume and losses (see render_backward).  `step` takes marched samples;
     `step_rays` takes the rays and marches them inside the backward kernel (three launches)."""
 
     def __init__(self, network_fn, volume, imgs, pose_ref, lr=5e-4, betas=(0.9, 0.999), eps=1e-8, white_bkgd=False,
                  grad_mode=_lib.MLP_FP32):
-        _check_grad_mode(grad_mode)
+        _check_grad_mode(grad_mode, rays=True)
         self.grad_mode = grad_mode
         self.network_fn, self.volume, self.imgs, self.pose_ref = network_fn, volume, imgs, pose_ref
         self.lr, self.betas, self.eps, self.white_bkgd = float(lr), (float(betas[0]), float(betas[1])), float(eps), bool(white_bkgd)
@@ -877,6 +888,7 @@ class FineTuner:
     def step(self, rays_pts, rays_ndc, z_vals, rays_dir, target_rgb, lr=None, want_forward=False):
         """One optimisation step on a batch.  Returns (loss [1] device tensor -- img2mse of this batch BEFORE the
         update, as the reference logs it -- and (rgb, depth) of the forward pass when `want_forward`)."""
+        _check_grad_mode(self.grad_mode)
         lr = self.lr if lr is None else float(lr)
         self.step_count += 1
         self.loss.zero_()

@@ -427,7 +427,7 @@ size_t mvsn_render_backward_workspace_bytes(int N, int S) { return render_backwa
 size_t mvsn_render_backward_tc_workspace_bytes(int N, int S) { return render_backward_tc_workspace_bytes(N, S); }
 size_t mvsn_render_backward_deterministic_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode) {
     if (grad_mode != MVSN_MLP_FP32 && grad_mode != MVSN_MLP_TC_HALF) return 0;
-    return render_backward_det_workspace_bytes(N, S, D, Hp, Wp, grad_mode == MVSN_MLP_TC_HALF);
+    return render_backward_det_workspace_bytes(N, S, D, Hp, Wp, grad_mode);
 }
 
 static int render_backward_entry(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
@@ -453,7 +453,7 @@ static int render_backward_entry(const mvsn_render_scene* scene, const float* co
     return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
                                   g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
                                   grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
-                                  (cudaStream_t)stream, tc, det);
+                                  (cudaStream_t)stream, tc ? MVSN_MLP_TC_HALF : MVSN_MLP_FP32, det);
 }
 
 int mvsn_render_backward(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
@@ -485,11 +485,15 @@ int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const flo
                                  workspace, workspace_bytes, stream, grad_mode == MVSN_MLP_TC_HALF, true);
 }
 
+// the grad modes of the rays entries
+static bool rays_grad_mode(int grad_mode) {
+    return grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF || grad_mode == MVSN_GRAD_TC_FULL;
+}
+
 size_t mvsn_render_backward_rays_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
-    if (grad_mode != MVSN_MLP_FP32 && grad_mode != MVSN_MLP_TC_HALF) return 0;
-    const bool tc = grad_mode == MVSN_MLP_TC_HALF;
-    if (deterministic) return render_backward_det_workspace_bytes(N, S, D, Hp, Wp, tc);
-    return tc ? render_backward_tc_workspace_bytes(N, S) : render_backward_workspace_bytes(N, S);
+    if (!rays_grad_mode(grad_mode)) return 0;
+    if (deterministic) return render_backward_det_workspace_bytes(N, S, D, Hp, Wp, grad_mode);
+    return render_backward_mode_workspace_bytes(N, S, grad_mode);
 }
 
 // mvsn_render_backward_rays and, with `stop`, mvsn_render_backward_rays_stop (`what`: the entry's name for messages)
@@ -498,8 +502,8 @@ static int backward_rays_entry(const char* what, const mvsn_render_scene* scene,
                                int N, int S, int grad_mode, int deterministic, const mvsn_render_grads* g,
                                float* const* grad_mlp, float* grad_volume_dhwc, void* workspace, size_t workspace_bytes,
                                void* stream, const BwdStop* stop) {
-    MVSN_REQUIRE(grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF, MVSN_EUNSUPPORTED,
-                 "%s: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)", what, grad_mode);
+    MVSN_REQUIRE(rays_grad_mode(grad_mode), MVSN_EUNSUPPORTED,
+                 "%s: grad_mode %d (MVSN_MLP_FP32, MVSN_MLP_TC_HALF or MVSN_GRAD_TC_FULL)", what, grad_mode);
     SceneDev sc;
     int rc = make_scene(scene, sc);
     if (rc) return rc;
@@ -535,7 +539,7 @@ static int backward_rays_entry(const char* what, const mvsn_render_scene* scene,
     return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
                                   g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
                                   grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
-                                  (cudaStream_t)stream, grad_mode == MVSN_MLP_TC_HALF, deterministic != 0, jitter, stop);
+                                  (cudaStream_t)stream, grad_mode, deterministic != 0, jitter, stop);
 }
 
 int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
@@ -548,8 +552,8 @@ int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const
 }
 
 size_t mvsn_render_backward_rays_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
-    if (grad_mode != MVSN_MLP_FP32 && grad_mode != MVSN_MLP_TC_HALF) return 0;
-    return render_backward_stop_workspace_bytes(N, S, D, Hp, Wp, grad_mode == MVSN_MLP_TC_HALF, deterministic != 0);
+    if (!rays_grad_mode(grad_mode)) return 0;
+    return render_backward_stop_workspace_bytes(N, S, D, Hp, Wp, grad_mode, deterministic != 0);
 }
 
 int mvsn_render_backward_rays_stop(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,

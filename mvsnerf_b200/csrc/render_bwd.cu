@@ -27,6 +27,8 @@
 //
 // grad_mode MVSN_MLP_TC_HALF (mvsn_render_backward_tc) runs render_bwd_tc_kernel instead: the same tile with its
 // dgrad / wgrad GEMMs on wgmma with fp16 operands; its schedule and numerics are described above the kernel.
+// grad_mode MVSN_GRAD_TC_FULL (rays entries only) runs it with FULL = true: the forward recompute's MLP on wgmma too
+// (tile_mlp_tc, described above it).
 //
 // mvsn_render_backward_deterministic runs either kernel with DET = true: the volume scatter and the fused loss are
 // recorded instead of summed with float atomics, then summed in a fixed-point scatter and a fixed-order reduction
@@ -924,7 +926,274 @@ __device__ __forceinline__ void frag_load_rm(float (&acc)[8][8], const float* sr
     __syncthreads();
 }
 
-template <bool DET, bool FAST, bool STOP = false>
+// ============================== grad_mode MVSN_GRAD_TC_FULL: the forward recompute on wgmma too =====================
+// tile_mlp_tc replaces tile_mlp in render_bwd_tc_kernel<.., FULL = true> (the rays entries); the backward half of the
+// kernel is unchanged.  Arithmetic of the recompute's MLP:
+//   * GEMMs with N >= 64 on wgmma, fp16 operands, fp32 accumulation: pts_bias (K 20 -> 32), layer 0 (K 63 -> 64),
+//     layers 1-4, layer 5 (encoding 64 + h 128), feature_linear, and the 128 feature columns of views_linears.0.
+//   * Front-end operands (encoding, features) unscaled; hidden activations and f carry a power-of-two scale 2^e per
+//     sample row, its maximum |v| in [2^14, 2^15) (e = 0 for a zero row, clamped to +-62).  A row's result depends on
+//     that row only, so the STOP phase-B recompute repeats phase A bit for bit and a ray's outputs do not depend on the
+//     other rays of the batch.  Layer 5's encoding part is accumulated unscaled and the accumulator rows are then
+//     multiplied by 2^e (exact) before the h part.  Weights unscaled.  Conversions cvt.rn.satfinite.
+//   * The heads of width <= 3 (alpha_linear, rgb_linear, the view-direction columns of views_linears.0): FFMA on
+//     operands rounded as fp16 rounds them (round_half), as in the backward.
+//   * Biases, modulation product, ReLU, sigmoid, alpha, and everything outside the MLP: fp32.
+// Schedule: warpgroup wg owns rows [64 wg, 64 wg + 64); A operands live in registers in the accumulator layout (the
+// front-end ones are read from the fp32 rows in sm.pe / sm.h), so a layer's output converts straight into the next
+// layer's A.  B operands are the fp16 weight image (the dgrad image read K-major, plus W_0 / W_5P), streamed by
+// cp.async through three 32 KB buffers (sm.w and two in sm.mod), two loads ahead.  The tile leaves what tile_mlp
+// leaves: sigma / (r, g, b, alpha) per row, hv in sm.mod, and the ScratchRecord of this mode's fp32 values.
+namespace bwdtc {
+constexpr int W_0  = WIMG;                        // pts_linears.0.weight              [128][64] (k < 63)
+constexpr int W_5P = W_0 + 128 * 64;              // pts_linears.5.weight[:, :63]      [128][64] (k < 63)
+constexpr int WIMG_FULL = W_5P + 128 * 64;
+}  // namespace bwdtc
+
+__global__ void pack_fwd_half_kernel(MlpPtrsB w, __half* __restrict__ out) {
+    using namespace bwdtc;
+    const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
+    for (int i = tid; i < 128 * 64; i += nt) {
+        const int n = i >> 6, k = i & 63, o = core_off(n, k, 64);
+        out[W_0 + o] = to_half_sat(k < 63 ? w.p[0][n * 63 + k] : 0.f);
+        out[W_5P + o] = to_half_sat(k < 63 ? w.p[10][n * 191 + k] : 0.f);
+    }
+}
+
+// two fp32 -> packed fp16x2 (low half = first argument), saturating
+__device__ __forceinline__ uint32_t cvt_h2_satf(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;\n" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+// exponent e of a row's scale 2^e: m * 2^e in [2^14, 2^15) (block_scale_exp's rule, for one row)
+__device__ __forceinline__ int row_exp(float m) {
+    const unsigned b = __float_as_uint(m);
+    if (b == 0u) return 0;
+    const int e = 14 - ((int)(b >> 23) - 127);
+    return e < -62 ? -62 : (e > 62 ? 62 : e);
+}
+// accumulator v (v[i]: row a if (i & 2) == 0, else row b) -> the next GEMM's A registers, each row scaled to its own
+// exponent (ea / eb out); the four threads of a quad hold a whole row
+template <int NV>
+__device__ __forceinline__ void to_operand(const float (&v)[NV], uint32_t (&a)[NV / 2], int& ea, int& eb) {
+    float ma = 0.f, mb = 0.f;
+#pragma unroll
+    for (int i = 0; i < NV; i += 4) {
+        ma = fmaxf(ma, fmaxf(fabsf(v[i]), fabsf(v[i + 1])));
+        mb = fmaxf(mb, fmaxf(fabsf(v[i + 2]), fabsf(v[i + 3])));
+    }
+    ma = fmaxf(ma, __shfl_xor_sync(0xffffffffu, ma, 1)); ma = fmaxf(ma, __shfl_xor_sync(0xffffffffu, ma, 2));
+    mb = fmaxf(mb, __shfl_xor_sync(0xffffffffu, mb, 1)); mb = fmaxf(mb, __shfl_xor_sync(0xffffffffu, mb, 2));
+    ea = row_exp(ma); eb = row_exp(mb);
+    const float sa = exp2i(ea), sb = exp2i(eb);
+#pragma unroll
+    for (int i = 0; i < NV; i += 2) {
+        const float s = (i & 2) ? sb : sa;
+        a[i >> 1] = cvt_h2_satf(v[i] * s, v[i + 1] * s);
+    }
+}
+// KS K-steps of an unscaled fp32 front-end operand (rows of `src`, stride ld) -> A registers of the warpgroup's rows
+template <int KS>
+__device__ __forceinline__ void front_operand(uint32_t (&a)[KS * 4], const float* src, int ld, int tid) {
+    const int t = tid & 127, w = t >> 5, g = (t >> 2) & 7, q = t & 3, row = 64 * (tid >> 7) + 16 * w + g;
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float2 v = *reinterpret_cast<const float2*>(src + (row + 8 * (i & 1)) * ld + 16 * ks + 8 * (i >> 1) + 2 * q);
+            a[ks * 4 + i] = cvt_h2_satf(v.x, v.y);
+        }
+}
+// d (+)= A * W^T for the warpgroup's 64 rows: A from registers (KS K-steps), W [N][ldk] core-matrix tile in shared
+// memory read K-major (the B operand of the forward)
+template <int N, int KS>
+__device__ __forceinline__ void tc_fwd(float (&d)[N / 2], const uint32_t (&a)[KS * 4], const __half* w, int ldk, bool acc) {
+    const uint32_t sb = hop::smem_u32(w);
+    hop::wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks)
+        hop::Wgmma<N>::rs(d, a + 4 * ks, hop::desc_nosw(sb + ks * 256, 128, ldk * 16), (acc || ks > 0) ? 1 : 0);
+    hop::wgmma_commit();
+    hop::wgmma_wait<0>();
+    hop::reg_fence(d);
+}
+// the record of an N = 128 layer output: dstT[col][row] (128-float rows of the CTA's scratch)
+__device__ __forceinline__ void record_T(const float (&v)[64], float* dstT, int tid) {
+    const int t = tid & 127, w = t >> 5, g = (t >> 2) & 7, q = t & 3, row = 64 * (tid >> 7) + 16 * w + g;
+#pragma unroll
+    for (int i = 0; i < 64; ++i) dstT[(8 * (i >> 2) + 2 * q + (i & 1)) * 128 + row + 8 * ((i >> 1) & 1)] = v[i];
+}
+// cp.async weight loads up to the last N outstanding are complete and visible to wgmma, and every thread is past
+// the GEMMs before this barrier
+template <int N>
+__device__ __forceinline__ void load_w_ready() {
+    cp_async_wait<N>();
+    hop::fence_proxy_async();
+    __syncthreads();
+}
+
+// The forward MLP of a tile whose front end is complete (all 256 threads, after the barrier behind the front end).
+// Leaves sm.sig, sm.rgb (written by the quad's first thread of each row), hv in sm.mod [128][HV_LD], and the
+// ScratchRecord (S_MODT, S_HT, S_FT) in scr; no closing barrier.
+__device__ __forceinline__ void tile_mlp_tc(const TileSmem& sm, const float* __restrict__ wts, const __half* __restrict__ wh,
+                                            float* scr, int tid) {
+    using namespace bwdtc;
+    const int t = tid & 127, w = t >> 5, g = (t >> 2) & 7, q = t & 3;
+    const int row_a = 64 * (tid >> 7) + 16 * w + g, row_b = row_a + 8;
+    __half* const buf0 = reinterpret_cast<__half*>(sm.w);
+    __half* const buf1 = reinterpret_cast<__half*>(sm.mod);
+    __half* const buf2 = buf1 + 128 * 128;
+    auto bias2 = [&](int base, int j) { return __ldg(reinterpret_cast<const float2*>(wts + base + 8 * j + 2 * q)); };
+    float acc[64], mod[64];
+    uint32_t a[32];
+    int ea = 0, eb = 0;
+    // the epilogue of a trunk layer: h = relu((acc 2^-e + b) * mod), recorded; then the next A operand
+    auto trunk_epilogue = [&](int bias, int l) {
+        const float ia = exp2i(-ea), ib = exp2i(-eb);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const float2 b = bias2(bias, j);
+#pragma unroll
+            for (int i = 4 * j; i < 4 * j + 4; ++i)
+                acc[i] = fmaxf((acc[i] * ((i & 2) ? ib : ia) + ((i & 1) ? b.y : b.x)) * mod[i], 0.f);
+        }
+        record_T(acc, scr + bwd::S_HT + l * 16384, tid);
+        to_operand(acc, a, ea, eb);
+    };
+
+    load_w_issue(wh + W_B, 128 * 64, buf0, tid);                   // the weight stream: load i -> buffer i % 3
+    load_w_issue(wh + W_0, 128 * 64, buf1, tid);
+    {                                                               // modulation = pts_bias(feat) + bb (K 32)
+        uint32_t af[8];
+        front_operand<2>(af, sm.h, FEAT_LD, tid);
+        load_w_ready<1>();
+        load_w_issue(wh + W_14, 128 * 128, buf2, tid);
+        tc_fwd<128, 2>(acc, af, buf0, 64, false);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const float2 b = bias2(w32::BB, j);
+#pragma unroll
+            for (int i = 4 * j; i < 4 * j + 4; ++i) mod[i] = acc[i] + ((i & 1) ? b.y : b.x);
+        }
+        record_T(mod, scr + bwd::S_MODT, tid);
+    }
+    {                                                               // layer 0: encoding (K 64)
+        uint32_t ap[16];
+        front_operand<4>(ap, sm.pe, PE_LD, tid);
+        load_w_ready<1>();
+        load_w_issue(wh + W_14 + 16384, 128 * 128, buf0, tid);
+        tc_fwd<128, 4>(acc, ap, buf1, 64, false);
+        ea = eb = 0;
+        trunk_epilogue(w32::B0, 0);
+    }
+#pragma unroll 1
+    for (int l = 1; l <= 4; ++l) {                                  // layers 1..4: load l + 1 in buffer (l + 1) % 3
+        load_w_ready<1>();
+        if (l <= 2) load_w_issue(wh + W_14 + (l + 1) * 16384, 128 * 128, l == 1 ? buf1 : buf2, tid);
+        else        load_w_issue(wh + (l == 3 ? W_5P : W_5H), l == 3 ? 128 * 64 : 128 * 128, l == 3 ? buf0 : buf1, tid);
+        const int nb = (l + 1) % 3;
+        tc_fwd<128, 8>(acc, a, nb == 0 ? buf0 : nb == 1 ? buf1 : buf2, 128, false);
+        trunk_epilogue(w32::W1 + (l - 1) * w32::LSTR + 128 * 128, l);
+    }
+    {                                                               // layer 5: [encoding | h] (skip connection)
+        uint32_t ap[16];
+        front_operand<4>(ap, sm.pe, PE_LD, tid);
+        load_w_ready<1>();                                          // load 6: W_5P in buf0
+        load_w_issue(wh + W_F, 128 * 128, buf2, tid);
+        tc_fwd<128, 4>(acc, ap, buf0, 64, false);
+        const float sa = exp2i(ea), sb = exp2i(eb);                 // to the scale of the h rows (exact)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] *= (i & 2) ? sb : sa;
+        load_w_ready<1>();                                          // load 7: W_5H in buf1
+        load_w_issue(wh + W_VF, 64 * 128, buf0, tid);
+        tc_fwd<128, 8>(acc, a, buf1, 128, true);
+        trunk_epilogue(w32::B5, 5);
+    }
+    float sig_a, sig_b;
+    {                                                               // sigma = relu(alpha_linear(h6)): FFMA, round_half
+        float pa = 0.f, pb = 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const float2 wa = bias2(w32::WA, j);
+            const float w0 = round_half(wa.x), w1 = round_half(wa.y);
+            // h6 = the record just written; acc still holds it
+            pa = fmaf(round_half(acc[4 * j]), w0, pa); pa = fmaf(round_half(acc[4 * j + 1]), w1, pa);
+            pb = fmaf(round_half(acc[4 * j + 2]), w0, pb); pb = fmaf(round_half(acc[4 * j + 3]), w1, pb);
+        }
+        pa += __shfl_xor_sync(0xffffffffu, pa, 1); pa += __shfl_xor_sync(0xffffffffu, pa, 2);
+        pb += __shfl_xor_sync(0xffffffffu, pb, 1); pb += __shfl_xor_sync(0xffffffffu, pb, 2);
+        const float ba = __ldg(wts + w32::BA);
+        sig_a = fmaxf(pa + ba, 0.f); sig_b = fmaxf(pb + ba, 0.f);
+        if (q == 0) { sm.sig[row_a] = sig_a; sm.sig[row_b] = sig_b; }
+    }
+    {                                                               // f = feature_linear(h6)
+        load_w_ready<1>();                                          // load 8: W_F in buf2
+        tc_fwd<128, 8>(acc, a, buf2, 128, false);
+        const float ia = exp2i(-ea), ib = exp2i(-eb);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const float2 b = bias2(w32::BF, j);
+#pragma unroll
+            for (int i = 4 * j; i < 4 * j + 4; ++i) acc[i] = acc[i] * ((i & 2) ? ib : ia) + ((i & 1) ? b.y : b.x);
+        }
+        record_T(acc, scr + bwd::S_FT, tid);
+        to_operand(acc, a, ea, eb);
+    }
+    {                                                               // hv = relu(views_linears.0([f, dir])), rgb, alpha
+        float hv[32];
+        load_w_ready<0>();                                          // load 9: W_VF in buf0; sm.mod is free after this
+        tc_fwd<64, 8>(hv, a, buf0, 128, false);
+        const float ia = exp2i(-ea), ib = exp2i(-eb);
+        float da[3], db[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) { da[c] = round_half(sm.dir[row_a * 4 + c]); db[c] = round_half(sm.dir[row_b * 4 + c]); }
+        float ra[3] = {0.f, 0.f, 0.f}, rb[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float2 bv = bias2(w32::BV, j);
+            float2 wd[3], wr[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                wd[c] = bias2(w32::WVD + c * 64, j); wd[c].x = round_half(wd[c].x); wd[c].y = round_half(wd[c].y);
+                wr[c] = bias2(w32::WR + c * 64, j); wr[c].x = round_half(wr[c].x); wr[c].y = round_half(wr[c].y);
+            }
+#pragma unroll
+            for (int i = 4 * j; i < 4 * j + 4; ++i) {
+                const bool hi = i & 1, rb_ = i & 2;
+                const float* d = rb_ ? db : da;
+                float v = hv[i] * (rb_ ? ib : ia);
+                v = fmaf(d[2], hi ? wd[2].y : wd[2].x, fmaf(d[1], hi ? wd[1].y : wd[1].x, fmaf(d[0], hi ? wd[0].y : wd[0].x, v)));
+                v = fmaxf(v + (hi ? bv.y : bv.x), 0.f);
+                hv[i] = v;
+                const float vr = round_half(v);
+                float* r = rb_ ? rb : ra;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) r[c] = fmaf(vr, hi ? wr[c].y : wr[c].x, r[c]);
+            }
+            const int col = 8 * j + 2 * q;
+            *reinterpret_cast<float2*>(sm.mod + row_a * HV_LD + col) = make_float2(hv[4 * j], hv[4 * j + 1]);
+            *reinterpret_cast<float2*>(sm.mod + row_b * HV_LD + col) = make_float2(hv[4 * j + 2], hv[4 * j + 3]);
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            ra[c] += __shfl_xor_sync(0xffffffffu, ra[c], 1); ra[c] += __shfl_xor_sync(0xffffffffu, ra[c], 2);
+            rb[c] += __shfl_xor_sync(0xffffffffu, rb[c], 1); rb[c] += __shfl_xor_sync(0xffffffffu, rb[c], 2);
+        }
+        if (q == 0) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float br = __ldg(wts + w32::BR + c);
+                sm.rgb[row_a * 4 + c] = __fdiv_rn(1.f, 1.f + expf(-(ra[c] + br)));
+                sm.rgb[row_b * 4 + c] = __fdiv_rn(1.f, 1.f + expf(-(rb[c] + br)));
+            }
+            sm.rgb[row_a * 4 + 3] = 1.f - expf(-sig_a);
+            sm.rgb[row_b * 4 + 3] = 1.f - expf(-sig_b);
+        }
+    }
+}
+
+template <bool DET, bool FAST, bool STOP = false, bool FULL = false>
 __global__ void __launch_bounds__(256, 1)
 render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const float* __restrict__ wts,
                      const __half* __restrict__ wh, const DetIO det, const float* __restrict__ jitter, const StopIO stop) {
@@ -958,7 +1227,7 @@ render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const
 
     for (int grp = blockIdx.x; STOP || grp < ngroups; grp += gridDim.x) {
         if constexpr (STOP) { if (!stop_next_tile(smem, stop, grp, ngroups, R, S, N, tid)) break; }
-        // =============================== forward recompute (the fp32 tile) ===========================
+        // =============================== forward recompute (the fp32 tile; FULL: tile_mlp_tc) ==========
         bool valid = false;
         size_t si = 0;
         if (tid < TILE_M) {
@@ -975,7 +1244,8 @@ render_bwd_tc_kernel(const SceneDev sc, const RenderIO io, const BwdIO bw, const
             }
         }
         __syncthreads();
-        tile_mlp(sm, wts, tid, ScratchRecord{scr});
+        if constexpr (FULL) tile_mlp_tc(sm, wts, wh, scr, tid);
+        else tile_mlp(sm, wts, tid, ScratchRecord{scr});
         __syncthreads();
         composite_scan<DET, STOP>(sc, bw, sm, s_T, s_g, grp, R, S, N, tid, det, &stop, smem);
         if constexpr (STOP) {
@@ -1289,22 +1559,28 @@ static int bwd_grid(int N, int S) {
     return ngroups < sm_count() ? ngroups : sm_count();
 }
 
-// One backward-kernel launch of the variant (tc, DET, FAST, STOP); wh is the fp16 dgrad image (tc) or unused.
+// One backward-kernel launch of the variant (grad_mode, DET, FAST, STOP); wh is the fp16 weight image (tensor-core
+// modes) or unused.  MVSN_GRAD_TC_FULL exists for FAST only (the launcher rejects it otherwise).
 template <bool DET, bool FAST, bool STOP = false>
-static int launch_bwd_kernel(bool tc, int grid, const SceneDev& sc, const RenderIO& io, const BwdIO& bw, const float* wts,
-                             const __half* wh, const DetIO& dt, const float* jitter, cudaStream_t stream,
+static int launch_bwd_kernel(int grad_mode, int grid, const SceneDev& sc, const RenderIO& io, const BwdIO& bw,
+                             const float* wts, const __half* wh, const DetIO& dt, const float* jitter, cudaStream_t stream,
                              const StopIO& stop = StopIO{}) {
-    static bool attr_set[2][64] = {};
-    const void* kfn = tc ? (const void*)render_bwd_tc_kernel<DET, FAST, STOP> : (const void*)render_bwd_kernel<DET, FAST, STOP>;
+    static bool attr_set[3][64] = {};
+    const int v = grad_mode == MVSN_GRAD_TC_FULL ? 2 : grad_mode == MVSN_MLP_TC_HALF ? 1 : 0;
+    MVSN_REQUIRE(FAST || v < 2, MVSN_EUNSUPPORTED, "MVSN_GRAD_TC_FULL: rays entries only");
+    const void* kfn = (const void*)render_bwd_kernel<DET, FAST, STOP>;
+    if (v == 1) kfn = (const void*)render_bwd_tc_kernel<DET, FAST, STOP>;
+    if constexpr (FAST) { if (v == 2) kfn = (const void*)render_bwd_tc_kernel<DET, FAST, STOP, true>; }
     const size_t smem = BWD_SMEM_BYTES + (STOP ? STOP_SMEM_BYTES : 0);
     int dev = 0;
     MVSN_CUDA_CHECK(cudaGetDevice(&dev));
-    if (dev >= 64 || !attr_set[tc][dev]) {
+    if (dev >= 64 || !attr_set[v][dev]) {
         MVSN_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (dev < 64) attr_set[tc][dev] = true;
+        if (dev < 64) attr_set[v][dev] = true;
     }
-    if (tc) render_bwd_tc_kernel<DET, FAST, STOP><<<grid, 256, smem, stream>>>(sc, io, bw, wts, wh, dt, jitter, stop);
-    else    render_bwd_kernel<DET, FAST, STOP><<<grid, 256, smem, stream>>>(sc, io, bw, wts, dt, jitter, stop);
+    if (v == 1) render_bwd_tc_kernel<DET, FAST, STOP><<<grid, 256, smem, stream>>>(sc, io, bw, wts, wh, dt, jitter, stop);
+    else if (v == 0) render_bwd_kernel<DET, FAST, STOP><<<grid, 256, smem, stream>>>(sc, io, bw, wts, dt, jitter, stop);
+    else if constexpr (FAST) render_bwd_tc_kernel<DET, FAST, STOP, true><<<grid, 256, smem, stream>>>(sc, io, bw, wts, wh, dt, jitter, stop);
     MVSN_CUDA_CHECK(cudaGetLastError());
     return MVSN_OK;
 }
@@ -1321,6 +1597,20 @@ size_t render_backward_tc_workspace_bytes(int N, int S) {
     if (S <= 0 || S > TILE_M || N <= 0) return 0;
     const size_t ctas = (size_t)sm_count();
     return ctas * (bwd::SCRATCH + bwd::GRADS) * sizeof(float) + bwdtc::WIMG * sizeof(__half);
+}
+
+// MVSN_GRAD_TC_FULL: the TC_HALF workspace with the forward's two extra weight operands in the fp16 image
+static size_t render_backward_tcf_workspace_bytes(int N, int S) {
+    if (S <= 0 || S > TILE_M || N <= 0) return 0;
+    const size_t ctas = (size_t)sm_count();
+    return ctas * (bwd::SCRATCH + bwd::GRADS) * sizeof(float) + bwdtc::WIMG_FULL * sizeof(__half);
+}
+
+// the workspace of a grad_mode's kernel (MVSN_MLP_FP32, MVSN_MLP_TC_HALF or MVSN_GRAD_TC_FULL)
+size_t render_backward_mode_workspace_bytes(int N, int S, int grad_mode) {
+    return grad_mode == MVSN_GRAD_TC_FULL ? render_backward_tcf_workspace_bytes(N, S)
+         : grad_mode == MVSN_MLP_TC_HALF  ? render_backward_tc_workspace_bytes(N, S)
+                                          : render_backward_workspace_bytes(N, S);
 }
 
 // Deterministic variant: the workspace of the grad mode, then (256-byte aligned) the [N] loss terms, and with a volume
@@ -1340,10 +1630,10 @@ DetLayout det_layout(size_t base, int N, int S, size_t nvox) {
 }
 }  // namespace
 
-size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc) {
+size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode) {
     const bool frozen = D == 0 && Hp == 0 && Wp == 0;
     if (!frozen && (D <= 0 || Hp <= 0 || Wp <= 0)) return 0;
-    const size_t base = tc ? render_backward_tc_workspace_bytes(N, S) : render_backward_workspace_bytes(N, S);
+    const size_t base = render_backward_mode_workspace_bytes(N, S, grad_mode);
     if (base == 0) return 0;
     return det_layout(base, N, S, (size_t)D * Hp * Wp).total;
 }
@@ -1364,9 +1654,9 @@ StopLayout stop_layout(size_t base, int N, int S) {
 }
 }  // namespace
 
-size_t render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc, bool det) {
-    const size_t base = det ? render_backward_det_workspace_bytes(N, S, D, Hp, Wp, tc)
-                            : (tc ? render_backward_tc_workspace_bytes(N, S) : render_backward_workspace_bytes(N, S));
+size_t render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, bool det) {
+    const size_t base = det ? render_backward_det_workspace_bytes(N, S, D, Hp, Wp, grad_mode)
+                            : render_backward_mode_workspace_bytes(N, S, grad_mode);
     return base ? stop_layout(base, N, S).total : 0;
 }
 
@@ -1374,14 +1664,16 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
                            const float* g_rgb, const float* target, float inv_count, const float* g_depth,
                            const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
                            float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det, const float* jitter,
+                           size_t workspace_bytes, cudaStream_t stream, int grad_mode, bool det, const float* jitter,
                            const BwdStop* stop) {
-    const bool fast = io.rays != nullptr;
+    const bool fast = io.rays != nullptr, tc = grad_mode != MVSN_MLP_FP32;
     const char* what = stop ? "mvsn_render_backward_rays_stop" : fast ? "mvsn_render_backward_rays"
                             : det ? (tc ? "deterministic render backward (grad_mode TC_HALF)" : "deterministic render backward")
                                   : (tc ? "render backward (grad_mode TC_HALF)" : "render backward");
     MVSN_REQUIRE(io.S <= TILE_M, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, io.S);
-    const size_t base = tc ? render_backward_tc_workspace_bytes(io.N, io.S) : render_backward_workspace_bytes(io.N, io.S);
+    MVSN_REQUIRE(fast || grad_mode != MVSN_GRAD_TC_FULL, MVSN_EUNSUPPORTED, "%s: MVSN_GRAD_TC_FULL is for the rays entries",
+                 what);
+    const size_t base = render_backward_mode_workspace_bytes(io.N, io.S, grad_mode);
     const size_t nvox = dvol ? (size_t)sc.D * sc.Hp * sc.Wp : 0;
     const DetLayout dl = det_layout(base, io.N, io.S, nvox);
     const StopLayout sl = stop_layout(det ? dl.total : base, io.N, io.S);
@@ -1412,6 +1704,10 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
     __half* wh = reinterpret_cast<__half*>(wimg);
     if (tc) {
         pack_dgrad_half_kernel<<<64, 256, 0, stream>>>(wp, wh);
+        if (grad_mode == MVSN_GRAD_TC_FULL) {
+            MVSN_CUDA_CHECK(cudaGetLastError());
+            pack_fwd_half_kernel<<<32, 256, 0, stream>>>(wp, wh);
+        }
     } else {
         bw.wd = wimg;
         pack_dgrad_kernel<<<64, 256, 0, stream>>>(wp, wimg);
@@ -1426,12 +1722,13 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
         st.list_cap = sl.list_cap;
         st.tiles_done = stop->tiles_done;
     }
-    const int rc = stop ? (det ? launch_bwd_kernel<true, true, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st)
-                               : launch_bwd_kernel<false, true, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st))
-                 : det ? (fast ? launch_bwd_kernel<true, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
-                               : launch_bwd_kernel<true, false>(tc, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream))
-                       : (fast ? launch_bwd_kernel<false, true>(tc, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
-                               : launch_bwd_kernel<false, false>(tc, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream));
+    const int gm = grad_mode;
+    const int rc = stop ? (det ? launch_bwd_kernel<true, true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st)
+                               : launch_bwd_kernel<false, true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st))
+                 : det ? (fast ? launch_bwd_kernel<true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
+                               : launch_bwd_kernel<true, false>(gm, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream))
+                       : (fast ? launch_bwd_kernel<false, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
+                               : launch_bwd_kernel<false, false>(gm, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream));
     if (rc) return rc;
     GradOut go;
     for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) go.p[i] = grad_mlp[i];

@@ -86,21 +86,23 @@ int launch_occupancy_ranges(const SceneDev& sc, const RenderIO& io, bool precise
 int launch_volume_to_half(const void* src, bool src_half, bool src_planar, long long nvox, void* dst, cudaStream_t stream);
 size_t mlp_wg_packed_bytes(bool split);
 int pack_mlp_wg(const float* const* w, bool split, void* packed, cudaStream_t stream);
-// fine-tuning step (render_bwd.cu); tc: dgrad / wgrad GEMMs on wgmma with fp16 operands (grad_mode TC_HALF);
+// fine-tuning step (render_bwd.cu); grad_mode: MVSN_MLP_FP32, MVSN_MLP_TC_HALF (dgrad / wgrad GEMMs on wgmma with
+// fp16 operands) or MVSN_GRAD_TC_FULL (TC_HALF plus the forward recompute's GEMMs on wgmma; io.rays entries only);
 // det: the volume gradient and the loss summed in a fixed order (bit-reproducible); io.rays set: the samples are
 // marched in the kernel from io.rays / io.t_steps, stratified by `jitter` [N,S] (NULL: none), instead of read from
 // io.pts / io.ndc / io.z / io.dirs
 size_t render_backward_workspace_bytes(int N, int S);
 size_t render_backward_tc_workspace_bytes(int N, int S);
-size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc);
-size_t render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, bool tc, bool det);
+size_t render_backward_mode_workspace_bytes(int N, int S, int grad_mode);
+size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode);
+size_t render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, bool det);
 // early ray termination of the rays backward (mvsn_render_backward_rays_stop); live_samples / tiles_done may be NULL
 struct BwdStop { float t_stop; int* live_samples; unsigned long long* tiles_done; };
 int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const float* const* mlp_w,
                            const float* g_rgb, const float* target, float inv_count, const float* g_depth,
                            const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
                            float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream, bool tc, bool det,
+                           size_t workspace_bytes, cudaStream_t stream, int grad_mode, bool det,
                            const float* jitter = nullptr, const BwdStop* stop = nullptr);
 int launch_adam_tensors(float* const* p, const float* const* g, float* const* m, float* const* v, const int* n, int count,
                         float lr, float beta1, float beta2, float eps, int step, cudaStream_t stream);

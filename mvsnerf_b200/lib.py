@@ -15,6 +15,7 @@ LIB_PATH = os.environ.get("MVSN_LIB") or os.path.join(HERE, "libmvsnerf_b200.so"
 
 MLP_FP32, MLP_TC_HALF, MLP_TC_SPLIT = 0, 1, 2
 MLP_TC_PAIR = 3          # same fp16-operand kernel as MLP_TC_HALF (csrc/render_wg.cu)
+GRAD_TC_FULL = 4         # grad_mode of the rays fine-tuning entries: TC_HALF's backward + the forward recompute on wgmma
 N_MLP_TENSORS, N_COSTREG_TENSORS, N_FEATURENET_TENSORS = 22, 30, 26
 
 # every symbol include/mvsnerf_b200.h declares (tests check the library exports all of them)

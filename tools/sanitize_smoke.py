@@ -103,9 +103,9 @@ if not only or "backward" in only:
             torch.use_deterministic_algorithms(False)
     # early ray termination (mvsn_render_backward_rays_stop): 400 rays x 128 samples = 400 one-ray groups on up to 132
     # CTAs, t_stop = 0.5 stops rays at different depths, so some tiles are back-propagated at once, others deferred, and
-    # a CTA's deferred rays fill packed tiles of which the last is partial; both grad modes and summation orders
+    # a CTA's deferred rays fill packed tiles of which the last is partial; every grad mode and summation order
     many = torch.cat([synthetic.scene_rays(sc)] * 2)[:400].contiguous().to(dev)
-    for mode in (lib.MLP_FP32, lib.MLP_TC_HALF):
+    for mode in (lib.MLP_FP32, lib.MLP_TC_HALF, lib.GRAD_TC_FULL):
         for det in (False, True):
             torch.use_deterministic_algorithms(det, warn_only=True)
             tiles = torch.zeros(3, dtype=torch.int64, device=dev)
@@ -114,6 +114,15 @@ if not only or "backward" in only:
                                          jitter=torch.rand(400, 128, device=dev), target_rgb=torch.rand(400, 3, device=dev),
                                          want_forward=True, grad_mode=mode, t_stop=0.5, live_samples=live, tiles_done=tiles)
             print("sanitize_smoke: backward stop", mode, det, "tiles", tiles.tolist())
+            torch.use_deterministic_algorithms(False)
+    # grad_mode GRAD_TC_FULL without early termination (mvsn_render_backward_rays), S 32 / 48 / 128, both orders
+    tuner = backend.FineTuner(fn, backend.RefVolume(vol.detach().clone()), d.imgs_raw, d.pose_source, lr=1e-4,
+                              grad_mode=lib.GRAD_TC_FULL)
+    for S in (32, 48, 128):
+        for det in (False, True):
+            torch.use_deterministic_algorithms(det, warn_only=True)
+            tuner.step_rays(rays[:37], torch.rand(37, 3, device=dev), sc.near_far, float(sc.pad), N_samples=S,
+                            want_forward=True)
             torch.use_deterministic_algorithms(False)
 torch.cuda.synchronize()
 print("sanitize_smoke: done")
