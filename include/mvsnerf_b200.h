@@ -133,6 +133,22 @@ int mvsn_render_samples(const mvsn_render_scene* scene,
                         float* rgb, float* depth, float* weights, float* alpha, float* input_feat,
                         void* stream);
 
+/* mvsn_render_samples_stop: mvsn_render_samples (rgb and depth only) with early ray termination, by the rule of
+ * mvsn_render_rays_stop: rays are composited in groups of up to 32 neighbours; after compositing tile k of a group, if
+ * every ray of the group has transmittance T < t_stop, the group's tiles k + 3 onwards are not computed and each pixel
+ * is the prefix of mvsn_render_samples' sums (same order, same arithmetic).  The omitted tail weighs less than t_stop:
+ * per channel, -t_stop < rgb - rgb_full <= 0 (white_bkgd: 0 <= rgb - rgb_full < t_stop), 0 <= depth_full - depth <
+ * t_stop * max z_vals.  t_stop = 0 never stops (bit-identical to mvsn_render_samples).  A group's result depends on its
+ * own rays only.  tiles_done (device, 8-byte aligned, may be NULL): += the number of 64-sample tiles computed.  Inputs
+ * as mvsn_render_samples; weights, alpha and input_feat are not computed (dead samples have none).
+ * Modes MVSN_MLP_TC_HALF / TC_PAIR / TC_SPLIT (optionally | MVSN_VOLUME_F16); MVSN_MLP_FP32 gives MVSN_EUNSUPPORTED.
+ * Argument errors (NULL pointers, t_stop negative or NaN, the mode, a misaligned tiles_done) are returned before any
+ * CUDA call. */
+int mvsn_render_samples_stop(const mvsn_render_scene* scene,
+                             const float* rays_pts, const float* rays_ndc, const float* z_vals,
+                             const float* rays_dir, int N, int S, float t_stop,
+                             float* rgb, float* depth, unsigned long long* tiles_done, void* stream);
+
 /* Fused-caller entry: also replaces data/ray_utils.ray_marcher (data/ray_utils.py:152-197,
  * perturb = 0) and utils.get_ndc_coordinate (utils.py:112-146) for the reference camera.
  *   rays [N,8] = (origin, direction, near, far); t_steps [S] = linspace(0,1,S) as the caller's
@@ -323,6 +339,33 @@ int mvsn_render_backward_rays_stop(const mvsn_render_scene* scene, const float* 
                                    int grad_mode, int deterministic, float t_stop, const mvsn_render_grads* g,
                                    float* const* grad_mlp, float* grad_volume_dhwc, int* live_samples,
                                    unsigned long long* tiles_done, void* workspace, size_t workspace_bytes, void* stream);
+/* mvsn_render_backward_stop: mvsn_render_backward (grad_mode MVSN_MLP_FP32) or mvsn_render_backward_tc
+ * (MVSN_MLP_TC_HALF) with early ray termination, by the rule of mvsn_render_backward_rays_stop: for each ray, with
+ * alpha_j from the fp32 recompute, T_0 = 1 and T_{j+1} = T_j ((1 - alpha_j) + 1e-10) (the kernel's fp32 order), sample
+ * j is live iff T_j >= t_stop; the live samples are a prefix of length L (L >= 1).  The step renders, forms the loss of
+ * and exactly differentiates the truncated render sum_{j<L} w_j c_j (depth and white_bkgd likewise); dead samples get
+ * no gradient and no volume scatter.  Against the full render, per channel -t_stop < rgb - rgb_full <= 0 (white_bkgd:
+ * 0 <= rgb - rgb_full < t_stop) and 0 <= depth_full - depth < t_stop * max z_vals, up to a few ulps.  t_stop = 0 keeps
+ * every sample: every output is bit-identical to the entry without it (mvsn_render_backward / _tc, or
+ * mvsn_render_backward_deterministic with deterministic != 0).  With MVSN_MLP_FP32 a ray's rgb, depth and loss term do
+ * not depend on the other rays of the batch; the MLP gradients may differ from a differently packed batch in summation
+ * order only.  deterministic != 0: every output is a deterministic function of the inputs, summed as
+ * mvsn_render_backward_deterministic sums them.  Inputs, g, grad_mlp and grad_volume_dhwc as mvsn_render_backward;
+ * N_samples <= 128.  live_samples [N] int32 (device, 4-byte aligned, may be NULL): each ray's L.  tiles_done (device,
+ * 8-byte aligned, may be NULL): unsigned long long[3] += the 128-row tiles back-propagated immediately, deferred, and
+ * packed from deferred rays.  Argument errors are returned before any CUDA call: a grad_mode other than MVSN_MLP_FP32
+ * or MVSN_MLP_TC_HALF (MVSN_EUNSUPPORTED), NULL pointers, t_stop negative, NaN or > 1 (MVSN_EBADSHAPE), g->weights /
+ * g->alpha / g->input_feat set (MVSN_EUNSUPPORTED: per-sample cotangents of dead samples are not defined), a misaligned
+ * grad_volume_dhwc, live_samples or tiles_done, then N_samples > 128 (MVSN_EUNSUPPORTED).  Workspace:
+ * mvsn_render_backward_stop_workspace_bytes(N, S, D, Hp, Wp, grad_mode, deterministic) bytes, 16-byte aligned; the
+ * volume dims matter only with `deterministic` (D = Hp = Wp = 0: a frozen volume).  0 for an unknown grad_mode or
+ * shape. */
+size_t mvsn_render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic);
+int mvsn_render_backward_stop(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                              const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                              int grad_mode, int deterministic, float t_stop, const mvsn_render_grads* g,
+                              float* const* grad_mlp, float* grad_volume_dhwc, int* live_samples,
+                              unsigned long long* tiles_done, void* workspace, size_t workspace_bytes, void* stream);
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
                    const int* numel_host, int count, float lr, float beta1, float beta2, float eps, int step,
                    void* stream);

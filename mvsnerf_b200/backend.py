@@ -492,14 +492,35 @@ def rendering(args, pose_ref, rays_pts, rays_ndc, depth_candidates, rays_o, rays
     use_viewdirs, raw_noise_std, NDC_local) are accepted and ignored, as the reference does.
     `mlp_mode=` selects the GEMM arithmetic (default: DEFAULT_MLP_MODE, the fp32-grade tensor mode); `want_aux=False` skips the three
     per-sample outputs (they are returned as None).  Under autograd, `grad_mode=` selects the arithmetic of the backward's
-    GEMMs (see render_backward; default MLP_FP32)."""
+    GEMMs (see render_backward; default MLP_FP32).
+
+    `t_stop=` (a float >= 0, tensor-core mlp_mode; None, the default, changes nothing): early ray termination
+    (mvsn_render_samples_stop) -- a group of up to 32 neighbouring rays stops two tiles after every ray in it has
+    transmittance < t_stop, so each channel of rgb differs from the full render by less than t_stop and depth by less
+    than t_stop * max(z) (t_stop = 0: bit-identical).  The samples behind are not computed, so the three per-sample
+    outputs (input_feat, weights, alpha) are returned as None.  `tiles_done=`: an optional CUDA int64 tensor [1] the
+    number of computed 64-sample tiles is added to.  Under autograd t_stop must lie in [0, 1]; the backward is
+    render_backward(..., t_stop=t_stop) with the rgb and depth cotangents: each ray back-propagates the prefix of samples
+    whose transmittance in front of them is >= t_stop.  create_nerf_mvs puts `t_stop` into the render kwargs when the
+    caller's `args` has one."""
     if pose_ref is None or img_feat is not None or getattr(args, "use_color_volume", False):
         raise RuntimeError("rendering: only the pose_ref / image-gather branch of the reference is implemented "
                            "(use_color_volume=False, img_feat=None) -- the branch every shipped config uses")
     mode = kwargs.pop("mlp_mode", DEFAULT_MLP_MODE)
     want_aux = kwargs.pop("want_aux", True)
     grad_mode = kwargs.pop("grad_mode", _lib.MLP_FP32)
+    t_stop = kwargs.pop("t_stop", None)
+    tiles_done = kwargs.pop("tiles_done", None)
     _check_grad_mode(grad_mode)
+    if t_stop is not None:
+        t_stop = float(t_stop)
+        if not t_stop >= 0.0:
+            raise RuntimeError(f"rendering: t_stop={t_stop} must be >= 0")
+        if mode == _lib.MLP_FP32:
+            raise RuntimeError("rendering: t_stop needs a tensor-core mlp_mode (MLP_TC_HALF / TC_PAIR / TC_SPLIT)")
+        _check_counter(tiles_done, "rendering", "tiles_done", torch.int64, 1, rays_pts.device)
+    elif tiles_done is not None:
+        raise RuntimeError("rendering: tiles_done needs t_stop")
     N, S = rays_pts.shape[:2]
     z = depth_candidates.expand(N, S) if depth_candidates.shape != (N, S) else depth_candidates
     vol_t = volume_feature.feat_volume if isinstance(volume_feature, nn.Module) else volume_feature
@@ -507,19 +528,32 @@ def rendering(args, pose_ref, rays_pts, rays_ndc, depth_candidates, rays_o, rays
         # training step (fine-tuning, train_mvs_nerf_finetuning_pl.py:164): same kernel forward, gradients for
         # the MLP parameters and the encoding volume (see _RenderSamplesFn)
         params = network_fn.ordered_params()
+        if t_stop is not None and t_stop > 1.0:
+            raise RuntimeError(f"rendering: t_stop={t_stop} must be in [0, 1] under autograd (see render_backward)")
+        stop = () if t_stop is None else ((t_stop, tiles_done),)
         rgb, feat, weights, depth, alpha = _RenderSamplesFn.apply(
             rays_pts, rays_ndc, z, rays_dir, vol_t, imgs, pose_ref["w2cs"], pose_ref["intrinsics"],
-            bool(white_bkgd), mode, network_fn, volume_feature, grad_mode, *params)
+            bool(white_bkgd), mode, network_fn, volume_feature, (grad_mode,) + stop, *params)
         return rgb, feat, weights, depth, alpha, {}
     rgb, feat, weights, depth, alpha = _render_samples_kernel(
         pose_ref, rays_pts, rays_ndc, z, rays_dir, volume_feature, imgs, network_fn, white_bkgd, mode, want_aux,
-        half_ok=True)
+        half_ok=True, t_stop=t_stop, tiles_done=tiles_done)
     return rgb, feat, weights, depth, alpha, {}
 
 
+def _check_counter(t, who, name, dtype, n, device):
+    """An optional output counter (live_samples / tiles_done): a contiguous CUDA `dtype` tensor of >= n elements on
+    `device`."""
+    if t is not None and (not t.is_cuda or t.device != device or t.dtype != dtype or t.numel() < n
+                          or not t.is_contiguous()):
+        raise RuntimeError(f"{who}: {name} must be a contiguous CUDA {dtype} tensor of >= {n} elements on the input's "
+                           f"device ({device})")
+
+
 def _render_samples_kernel(pose_ref, rays_pts, rays_ndc, z, rays_dir, volume_feature, imgs, network_fn, white_bkgd,
-                           mode, want_aux=True, half_ok=False):
-    """One mvsn_render_samples launch (no autograd graph); half_ok: see _make_scene."""
+                           mode, want_aux=True, half_ok=False, t_stop=None, tiles_done=None):
+    """One mvsn_render_samples launch (no autograd graph); half_ok: see _make_scene.  With `t_stop`: one
+    mvsn_render_samples_stop launch, and the per-sample outputs are None."""
     lib = _lib.load()
     N, S = rays_pts.shape[:2]
     dev = rays_pts.device
@@ -531,6 +565,13 @@ def _render_samples_kernel(pose_ref, rays_pts, rays_ndc, z, rays_dir, volume_fea
     rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
     depth = torch.empty(N, dtype=torch.float32, device=dev)
     feat = weights = alpha = None
+    if t_stop is not None:
+        with torch.cuda.device(dev):
+            _lib.check(lib.mvsn_render_samples_stop(C.byref(sc), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z), _lib.ptr(dirs),
+                                                    N, S, t_stop, _lib.ptr(rgb), _lib.ptr(depth), _lib.ptr(tiles_done),
+                                                    _lib.stream_ptr()), "mvsn_render_samples_stop")
+        del keep
+        return rgb, feat, weights, depth, alpha
     if want_aux:
         feat = torch.empty(N, S, 20, dtype=torch.float32, device=dev)
         weights = torch.empty(N, S, dtype=torch.float32, device=dev)
@@ -582,22 +623,43 @@ class _RenderSamplesFn(torch.autograd.Function):
     fp32 render kernel's own forward tile, MLP dgrad/wgrad in the arithmetic `grad_mode` selects, trilinear scatter
     into the volume gradient; bit-reproducible under torch.use_deterministic_algorithms(True), see render_backward).
     Otherwise the chunk is re-evaluated with PyTorch ops under autograd (_render_samples_torch); activation memory then
-    exists only during backward."""
+    exists only during backward.
+
+    `how` = (grad_mode,) or, with early ray termination, (grad_mode, (t_stop, tiles_done)): the forward is then
+    mvsn_render_samples_stop (the per-sample outputs are None) and the backward render_backward(..., t_stop=t_stop)
+    with the rgb and depth cotangents (the kernel path only; a non-zero per-sample cotangent raises)."""
 
     @staticmethod
     def forward(ctx, pts, ndc, z, rays_dir, vol, imgs, w2cs, intrinsics, white_bkgd, mode, network_fn, volume_feature,
-                grad_mode, *params):
+                how, *params):
         pose = {"w2cs": w2cs, "intrinsics": intrinsics}
-        out = _render_samples_kernel(pose, pts, ndc, z, rays_dir, volume_feature, imgs, network_fn, white_bkgd, mode)
+        grad_mode, stop = how[0], (how[1] if len(how) > 1 else (None, None))
+        kw = {} if stop[0] is None else {"t_stop": stop[0], "tiles_done": stop[1]}
+        out = _render_samples_kernel(pose, pts, ndc, z, rays_dir, volume_feature, imgs, network_fn, white_bkgd, mode, **kw)
         ctx.save_for_backward(pts, ndc, z, rays_dir, vol, imgs, w2cs, intrinsics, *params)
         ctx.white_bkgd, ctx.network_fn, ctx.volume_feature = white_bkgd, network_fn, volume_feature
-        ctx.grad_mode = grad_mode
+        ctx.grad_mode, ctx.t_stop = grad_mode, stop[0]
         return out
 
     @staticmethod
     def backward(ctx, g_rgb, g_feat, g_weights, g_depth, g_alpha):
         pts, ndc, z, rays_dir, vol, imgs, w2cs, intrinsics, *params = ctx.saved_tensors
         S = pts.shape[1]
+        if ctx.t_stop is not None:
+            # early ray termination: the truncated render of the kernel backward, which has no per-sample outputs
+            if any(g is not None and bool(g.any()) for g in (g_feat, g_weights, g_alpha)):
+                raise RuntimeError("rendering with t_stop: input_feat / weights / alpha are not computed for dead samples "
+                                   "and take no cotangent")
+            if S > 128 or BACKWARD_IMPL != "kernel":
+                raise RuntimeError(f"rendering with t_stop: the backward kernel takes N_samples <= 128 (got {S})")
+            need_vol = ctx.needs_input_grad[4]
+            g_params, dvol, _, _ = render_backward(
+                {"w2cs": w2cs, "intrinsics": intrinsics}, pts, ndc, z, rays_dir, ctx.volume_feature, imgs, ctx.network_fn,
+                ctx.white_bkgd, grads={"rgb": g_rgb, "depth": g_depth}, want_volume_grad=need_vol,
+                grad_mode=ctx.grad_mode, t_stop=ctx.t_stop)
+            g_vol = dvol.permute(3, 0, 1, 2).unsqueeze(0) if need_vol else None
+            g_params = [g if need else None for g, need in zip(g_params, ctx.needs_input_grad[13:])]
+            return (None, None, None, None, g_vol, None, None, None, None, None, None, None, None, *g_params)
         if S <= 128 and BACKWARD_IMPL == "kernel":
             # the hand-written backward kernel (csrc/render_bwd.cu): recompute + dgrad/wgrad + volume scatter
             need_vol = ctx.needs_input_grad[4]
@@ -666,7 +728,8 @@ def _backward_workspace(dev, N, S, grad_mode=_lib.MLP_FP32, det_volume=None):
 
 def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_feature, imgs, network_fn, white_bkgd=False,
                     grads=None, target_rgb=None, n_total=None, want_volume_grad=True, grad_volume=None, grad_mlp=None,
-                    want_forward=False, loss_out=None, grad_mode=_lib.MLP_FP32):
+                    want_forward=False, loss_out=None, grad_mode=_lib.MLP_FP32, t_stop=None, live_samples=None,
+                    tiles_done=None):
     """One mvsn_render_backward launch (grad_mode=MLP_FP32: fp32 FFMA GEMMs) or mvsn_render_backward_tc launch
     (grad_mode=MLP_TC_HALF: the dgrad / wgrad GEMMs on tensor cores with fp16 operands, fp32 accumulation; the forward
     recompute, and so rgb / depth / the loss, are the same fp32 tile and bit-identical).  Either `grads` (dict with 'rgb' and optionally 'depth', 'weights', 'alpha',
@@ -677,11 +740,30 @@ def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_featu
 
     With torch.use_deterministic_algorithms(True) in effect at call time the launch is
     mvsn_render_backward_deterministic instead (same grad_mode): the volume gradient and the fused loss are summed in
-    a fixed order, so every output is bit-reproducible; otherwise they are summed with float atomics."""
+    a fixed order, so every output is bit-reproducible; otherwise they are summed with float atomics.
+
+    `t_stop` (a float in [0, 1]): early ray termination (mvsn_render_backward_stop, same grad_mode and summation-order
+    dispatch) -- each ray keeps the prefix of samples whose transmittance in front of them is >= t_stop, and the step
+    renders, forms the loss of and exactly differentiates that truncated render; each channel differs from the full
+    render by less than t_stop (t_stop = 0: bit-identical to t_stop=None).  Per-sample cotangents (`grads` 'weights',
+    'alpha', 'input_feat') are rejected with it.  `live_samples`: an optional CUDA int32 tensor [N] that receives each
+    ray's number of kept samples; `tiles_done`: an optional CUDA int64 tensor [3] the counts of tiles back-propagated
+    immediately, deferred and packed are added to."""
     _check_grad_mode(grad_mode)
-    lib = _lib.load()
     N, S = rays_pts.shape[:2]
     dev = rays_pts.device
+    if t_stop is not None:
+        t_stop = float(t_stop)
+        if not 0.0 <= t_stop <= 1.0:
+            raise RuntimeError(f"render_backward: t_stop={t_stop} must be in [0, 1]")
+        if grads is not None and any(grads.get(k) is not None for k in ("weights", "alpha", "input_feat")):
+            raise RuntimeError("render_backward: t_stop takes no per-sample cotangents (weights / alpha / input_feat):"
+                               " dead samples have none")
+        _check_counter(live_samples, "render_backward", "live_samples", torch.int32, N, dev)
+        _check_counter(tiles_done, "render_backward", "tiles_done", torch.int64, 3, dev)
+    elif live_samples is not None or tiles_done is not None:
+        raise RuntimeError("render_backward: live_samples / tiles_done need t_stop")
+    lib = _lib.load()
     pts = _lib.dev_f32(rays_pts.detach(), "rays_pts")
     ndc = _lib.dev_f32(rays_ndc.detach(), "rays_ndc")
     z = _lib.dev_f32((z_vals.expand(N, S) if z_vals.shape != (N, S) else z_vals).detach(), "depth_candidates")
@@ -694,6 +776,23 @@ def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_featu
         grad_volume = torch.zeros(sc.D, sc.Hp, sc.Wp, 8, dtype=torch.float32, device=dev)
     g, held, rgb, depth = _render_grads(N, S, dev, grads, target_rgb, n_total, want_forward, loss_out)
     vol_arg = _lib.ptr(grad_volume) if want_volume_grad else None
+    if t_stop is not None:
+        det = torch.are_deterministic_algorithms_enabled()
+        dims = (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0)
+        need = lib.mvsn_render_backward_stop_workspace_bytes(int(N), int(S), *dims, int(grad_mode), int(det))
+        if need == 0:
+            raise RuntimeError(f"render backward: unsupported shape N={N}, N_samples={S} (N_samples <= 128)")
+        ws = _bwd_workspace.get(dev)
+        if ws is None or ws.numel() < need:
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            _bwd_workspace[dev] = ws
+        with torch.cuda.device(dev):
+            _lib.check(lib.mvsn_render_backward_stop(
+                C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z), _lib.ptr(dirs), N, S,
+                int(grad_mode), int(det), t_stop, C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(live_samples),
+                _lib.ptr(tiles_done), _lib.ptr(ws), need, _lib.stream_ptr()), "mvsn_render_backward_stop")
+        del keep, held
+        return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
     if torch.are_deterministic_algorithms_enabled():
         ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode, (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0))
         with torch.cuda.device(dev):
@@ -885,9 +984,11 @@ class FineTuner:
         self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
         self._numel = (C.c_int * len(self.params))(*[p.numel() for p in self.params])
 
-    def step(self, rays_pts, rays_ndc, z_vals, rays_dir, target_rgb, lr=None, want_forward=False):
+    def step(self, rays_pts, rays_ndc, z_vals, rays_dir, target_rgb, lr=None, want_forward=False, t_stop=None):
         """One optimisation step on a batch.  Returns (loss [1] device tensor -- img2mse of this batch BEFORE the
-        update, as the reference logs it -- and (rgb, depth) of the forward pass when `want_forward`)."""
+        update, as the reference logs it -- and (rgb, depth) of the forward pass when `want_forward`).  `t_stop`: early
+        ray termination, as in render_backward -- the step trains the render truncated where each ray's transmittance
+        falls below t_stop, and skips the work of the samples behind."""
         _check_grad_mode(self.grad_mode)
         lr = self.lr if lr is None else float(lr)
         self.step_count += 1
@@ -895,7 +996,7 @@ class FineTuner:
         _, _, rgb, depth = render_backward(self.pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, self.volume, self.imgs,
                                            self.network_fn, self.white_bkgd, target_rgb=target_rgb, want_volume_grad=True,
                                            grad_volume=self.vol_g, grad_mlp=self.g, want_forward=want_forward,
-                                           loss_out=self.loss, grad_mode=self.grad_mode)
+                                           loss_out=self.loss, grad_mode=self.grad_mode, t_stop=t_stop)
         self._adam(lr)
         return self.loss, (rgb, depth)
 
@@ -1334,7 +1435,9 @@ def _network_query(pts, viewdirs, rays_feats, network_fn, netchunk=1024):
 
 def create_nerf_mvs(args, pts_embedder=True, use_mvs=False, dir_embedder=True, device=None):
     """Same contract as models.create_nerf_mvs: returns
-    (render_kwargs_train, render_kwargs_test, start, grad_vars)."""
+    (render_kwargs_train, render_kwargs_test, start, grad_vars).  When `args` has a `t_stop` attribute that is not
+    None, both kwargs dicts also carry it, so `rendering(args, ..., **render_kwargs)` runs with early ray termination
+    (see rendering); otherwise the dicts are exactly the reference's."""
     if not pts_embedder or dir_embedder:
         raise RuntimeError("create_nerf_mvs: the fused kernel implements pts_embedder=True, dir_embedder=False "
                            "(the combination every shipped caller uses)")
@@ -1365,6 +1468,8 @@ def create_nerf_mvs(args, pts_embedder=True, use_mvs=False, dir_embedder=True, d
         "N_samples": args.N_samples, "network_fn": model, "network_mvs": encoding_net,
         "use_viewdirs": args.use_viewdirs, "white_bkgd": args.white_bkgd, "raw_noise_std": args.raw_noise_std,
     }
+    if getattr(args, "t_stop", None) is not None:
+        render_kwargs_train["t_stop"] = float(args.t_stop)
     render_kwargs_test = dict(render_kwargs_train)
     render_kwargs_test["perturb"] = False
     return render_kwargs_train, render_kwargs_test, 0, grad_vars

@@ -259,6 +259,31 @@ int mvsn_render_samples(const mvsn_render_scene* scene, const float* rays_pts, c
     return dispatch_render(scene, sc, io, false, (cudaStream_t)stream);
 }
 
+int mvsn_render_samples_stop(const mvsn_render_scene* scene, const float* rays_pts, const float* rays_ndc,
+                             const float* z_vals, const float* rays_dir, int N, int S, float t_stop, float* rgb,
+                             float* depth, unsigned long long* tiles_done, void* stream) {
+    MVSN_RANGE("mvsn_render_samples_stop");
+    const char* what = "mvsn_render_samples_stop";
+    SceneDev sc;
+    int rc = make_scene(scene, sc);
+    if (rc) return rc;
+    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "%s: N=%d S=%d", what, N, S);
+    MVSN_REQUIRE(rays_pts && rays_ndc && z_vals && rays_dir && rgb && depth, MVSN_ENULL, "%s: NULL required pointer", what);
+    MVSN_REQUIRE(t_stop >= 0.f, MVSN_EBADSHAPE, "%s: t_stop=%g must be >= 0 (not NaN)", what, (double)t_stop);
+    const int mode = mlp_mode_of(scene);
+    MVSN_REQUIRE(mode == MVSN_MLP_TC_HALF || mode == MVSN_MLP_TC_PAIR || mode == MVSN_MLP_TC_SPLIT,
+                 MVSN_EUNSUPPORTED, "%s: mlp_mode %d has no early ray termination (tensor-core modes only)", what,
+                 scene->mlp_mode);
+    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(tiles_done) % 8 == 0, MVSN_EALIGN, "%s: tiles_done must be 8-byte aligned", what);
+    if (N == 0) return MVSN_OK;
+    RenderIO io{};
+    io.pts = rays_pts; io.ndc = rays_ndc; io.z = z_vals; io.dirs = rays_dir;
+    io.N = N; io.S = S;
+    io.rgb = rgb; io.depth = depth;
+    return launch_render_wg(sc, io, false, mode == MVSN_MLP_TC_SPLIT, scene->mlp_packed, (cudaStream_t)stream, &t_stop,
+                            tiles_done, half_volume(scene), nullptr, nullptr);
+}
+
 // host-side scalars of the in-kernel ray march exactly as utils.get_ndc_coordinate forms them (python floats -> fp32)
 static RayGenDev make_ray_gen(const mvsn_render_scene* scene, const mvsn_ray_params* rp) {
     RayGenDev rg;
@@ -483,6 +508,54 @@ int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const flo
                  "mvsn_render_backward_deterministic: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)", grad_mode);
     return render_backward_entry(scene, mlp_w, rays_pts, rays_ndc, z_vals, rays_dir, N, S, g, grad_mlp, grad_volume_dhwc,
                                  workspace, workspace_bytes, stream, grad_mode == MVSN_MLP_TC_HALF, true);
+}
+
+// the grad modes of the samples entries
+static bool samples_grad_mode(int grad_mode) { return grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF; }
+
+size_t mvsn_render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
+    if (!samples_grad_mode(grad_mode)) return 0;
+    return render_backward_stop_workspace_bytes(N, S, D, Hp, Wp, grad_mode, deterministic != 0);
+}
+
+int mvsn_render_backward_stop(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                              const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                              int grad_mode, int deterministic, float t_stop, const mvsn_render_grads* g,
+                              float* const* grad_mlp, float* grad_volume_dhwc, int* live_samples,
+                              unsigned long long* tiles_done, void* workspace, size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward_stop");
+    const char* what = "mvsn_render_backward_stop";
+    MVSN_REQUIRE(samples_grad_mode(grad_mode), MVSN_EUNSUPPORTED, "%s: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)",
+                 what, grad_mode);
+    SceneDev sc;
+    int rc = make_scene(scene, sc);
+    if (rc) return rc;
+    MVSN_REQUIRE(g && mlp_w && grad_mlp, MVSN_ENULL, "%s: NULL argument", what);
+    MVSN_REQUIRE(g->rgb || g->target_rgb, MVSN_ENULL, "%s: neither g->rgb nor g->target_rgb given", what);
+    for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i)
+        MVSN_REQUIRE(mlp_w[i] && grad_mlp[i], MVSN_ENULL, "%s: tensor %d is NULL", what, i);
+    MVSN_REQUIRE(N == 0 || (rays_pts && rays_ndc && z_vals && rays_dir), MVSN_ENULL, "%s: NULL required pointer", what);
+    MVSN_REQUIRE(t_stop >= 0.f && t_stop <= 1.f, MVSN_EBADSHAPE, "%s: t_stop=%g must be in [0, 1] (not NaN)", what,
+                 (double)t_stop);
+    MVSN_REQUIRE(!g->weights && !g->alpha && !g->input_feat, MVSN_EUNSUPPORTED,
+                 "%s: g->weights / g->alpha / g->input_feat are per-sample cotangents, not defined for dead samples", what);
+    MVSN_REQUIRE(!grad_volume_dhwc || aligned16(grad_volume_dhwc), MVSN_EALIGN, "grad_volume_dhwc must be 16-byte aligned");
+    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(live_samples) % 4 == 0, MVSN_EALIGN, "%s: live_samples must be 4-byte aligned",
+                 what);
+    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(tiles_done) % 8 == 0, MVSN_EALIGN, "%s: tiles_done must be 8-byte aligned", what);
+    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "%s: N=%d S=%d", what, N, S);
+    MVSN_REQUIRE(S <= 128, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, S);
+    MVSN_REQUIRE(scene->mlp_mode == MVSN_MLP_FP32, MVSN_EUNSUPPORTED,
+                 "%s: scene->mlp_packed must be the MVSN_MLP_FP32 image (mode %d given)", what, scene->mlp_mode);
+    if (N == 0) return MVSN_OK;
+    RenderIO io{};
+    io.pts = rays_pts; io.ndc = rays_ndc; io.z = z_vals; io.dirs = rays_dir;
+    io.N = N; io.S = S;
+    const BwdStop stop{t_stop, live_samples, tiles_done};
+    return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
+                                  g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
+                                  grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
+                                  (cudaStream_t)stream, grad_mode, deterministic != 0, nullptr, &stop);
 }
 
 // the grad modes of the rays entries

@@ -37,6 +37,9 @@
 // mvsn_render_backward_rays runs any of these with FAST = true: the front end marches the samples from the rays, as
 // render_rays does, with stratified depths from a caller-drawn jitter (ray_z_jittered), instead of reading the
 // per-sample arrays of ray_marcher / get_ndc_coordinate.
+//
+// mvsn_render_backward_rays_stop (FAST = true) and mvsn_render_backward_stop (FAST = false, the per-sample arrays) run
+// the FP32 and TC_HALF kernels with STOP = true: early ray termination (described above StopTables).
 #include <cfloat>
 
 #include "tile_fp32.cuh"
@@ -104,7 +107,7 @@ struct DetIO {
     unsigned* amax;          // [2] max |g| over the finite recorded values (float bits), and a non-finite flag
 };
 
-// What the STOP = true kernels (mvsn_render_backward_rays_stop) take besides
+// What the STOP = true kernels (mvsn_render_backward_rays_stop, mvsn_render_backward_stop) take besides
 struct StopIO {
     float t_stop;                    // sample j of a ray is live iff its transmittance T_j >= t_stop
     int* live;                       // [N] live samples per ray (the caller's live_samples, or the workspace)
@@ -187,7 +190,7 @@ constexpr int BWD_SMEM_FLOATS = TILE_SMEM_FLOATS + TILE_M * 18;
 constexpr size_t BWD_SMEM_BYTES = BWD_SMEM_FLOATS * sizeof(float);
 static_assert(TILE_M * PE_LD >= 64 * H_LD, "peT staging [64][H_LD] must fit in the positional-encoding region");
 
-// ---- early ray termination (STOP = true, mvsn_render_backward_rays_stop) -----------------------------------------
+// ---- early ray termination (STOP = true, mvsn_render_backward_rays_stop / mvsn_render_backward_stop) ---------------
 // Sample j of a ray is live iff T_j >= t_stop (T_0 = 1, T_{j+1} = T_j ((1 - alpha_j) + 1e-10), the scan's fp32 order);
 // T never increases, so the live samples are a prefix of length L.  The kernel differentiates exactly the truncated
 // render sum_{j<L} w_j c_j: dead samples get s_g = 0 and no volume scatter.  Two phases in the persistent launch:
@@ -476,7 +479,7 @@ __device__ __forceinline__ void volume_scatter(const SceneDev& sc, const RenderI
 
 // FAST: the front end marches the samples from io.rays / io.t_steps (stratified by `jitter` [N,S] unless NULL) instead of
 // reading io.pts / io.ndc / io.z / io.dirs (mvsn_render_backward_rays); `jitter` is unused otherwise.
-// STOP (FAST only): early ray termination at stop.t_stop, in two phases (described above StopTables); the launch adds
+// STOP: early ray termination at stop.t_stop, in two phases (described above StopTables); the launch adds
 // STOP_SMEM_BYTES of dynamic shared memory for the tables.  `stop` is unused otherwise.
 template <bool DET, bool FAST, bool STOP = false>
 __global__ void __launch_bounds__(256, 1)
@@ -1480,7 +1483,7 @@ __device__ __forceinline__ int det_scale_exp(unsigned amax_bits, long long n) {
 
 // FAST (the rays entry): each sample's NDC is marched again from io.rays / io.t_steps / jitter by the function the
 // backward kernel's front end used (sample_point), so it has the same bits and needs no per-sample record.
-// STOP (FAST only): the samples j >= live[ray] are dead; their records were never written, so they are skipped.
+// STOP: the samples j >= live[ray] are dead; their records were never written, so they are skipped.
 template <bool FAST, bool STOP = false>
 __global__ void det_scatter_kernel(const SceneDev sc, const float* __restrict__ ndc, const float* __restrict__ rec,
                                    const unsigned* __restrict__ amax, long long nsamp,
@@ -1667,7 +1670,8 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
                            size_t workspace_bytes, cudaStream_t stream, int grad_mode, bool det, const float* jitter,
                            const BwdStop* stop) {
     const bool fast = io.rays != nullptr, tc = grad_mode != MVSN_MLP_FP32;
-    const char* what = stop ? "mvsn_render_backward_rays_stop" : fast ? "mvsn_render_backward_rays"
+    const char* what = stop ? (fast ? "mvsn_render_backward_rays_stop" : "mvsn_render_backward_stop")
+                     : fast ? "mvsn_render_backward_rays"
                             : det ? (tc ? "deterministic render backward (grad_mode TC_HALF)" : "deterministic render backward")
                                   : (tc ? "render backward (grad_mode TC_HALF)" : "render backward");
     MVSN_REQUIRE(io.S <= TILE_M, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, io.S);
@@ -1723,8 +1727,10 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
         st.tiles_done = stop->tiles_done;
     }
     const int gm = grad_mode;
-    const int rc = stop ? (det ? launch_bwd_kernel<true, true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st)
-                               : launch_bwd_kernel<false, true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st))
+    const int rc = stop ? (det ? (fast ? launch_bwd_kernel<true, true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st)
+                                       : launch_bwd_kernel<true, false, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream, st))
+                               : (fast ? launch_bwd_kernel<false, true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st)
+                                       : launch_bwd_kernel<false, false, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream, st)))
                  : det ? (fast ? launch_bwd_kernel<true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
                                : launch_bwd_kernel<true, false>(gm, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream))
                        : (fast ? launch_bwd_kernel<false, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
@@ -1738,8 +1744,10 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
         const long long nsamp = (long long)io.N * io.S;
         auto* acc = reinterpret_cast<unsigned long long*>(static_cast<char*>(workspace) + dl.acc);
         const int gs = cdiv(nsamp * 64, 256) < sm_count() * 16 ? cdiv(nsamp * 64, 256) : sm_count() * 16;
-        if (stop) det_scatter_kernel<true, true><<<gs, 256, 0, stream>>>(sc, nullptr, dt.rec, dt.amax, nsamp, acc, dvol, io,
-                                                                         jitter, st.live);
+        if (stop && fast) det_scatter_kernel<true, true><<<gs, 256, 0, stream>>>(sc, nullptr, dt.rec, dt.amax, nsamp, acc, dvol,
+                                                                                 io, jitter, st.live);
+        else if (stop) det_scatter_kernel<false, true><<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, dvol,
+                                                                              io, nullptr, st.live);
         else if (fast) det_scatter_kernel<true><<<gs, 256, 0, stream>>>(sc, nullptr, dt.rec, dt.amax, nsamp, acc, dvol, io,
                                                                        jitter, nullptr);
         else      det_scatter_kernel<false><<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, dvol, io, nullptr,

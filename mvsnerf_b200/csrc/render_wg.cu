@@ -416,7 +416,7 @@ __device__ __forceinline__ void front_end(const SceneDev& sc, const Cams& cams, 
 template <bool STOP> struct StopRegs { bool verdict = false, idle = false, last = false, first = true; uint32_t ncomp = 0; };
 template <> struct StopRegs<false> { static constexpr bool last = false; };
 
-// STOP (early ray termination, FAST only): after compositing tile k of a group, if every valid ray of the group has
+// STOP (early ray termination; the ray entry, FAST, and the samples entry): after compositing tile k of a group, if every valid ray of the group has
 // transmittance cT < t_stop, the group's tiles k + 3 onwards are not computed (k + 1 and k + 2 are composited as
 // usual), and the number of passes of a CTA becomes dynamic.  Each consumer computes its plan for pass p + 2 at the
 // start of pass p: the next tile of its group, or the next group of the CTA's list (a shared counter, in order of
@@ -923,7 +923,7 @@ render_wg_kernel(const SceneDev sc, const RenderIO io, const uint8_t* __restrict
     }
 }
 
-// the dynamic shared memory of the six instantiations with volume storage VT
+// the dynamic shared memory of the eight instantiations with volume storage VT
 template <typename VT>
 static int set_wg_smem_attributes() {
     using namespace wg;
@@ -935,6 +935,10 @@ static int set_wg_smem_attributes() {
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false, false) + STOP_BYTES));
     MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<true, true, true, VT, const int2*>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true, false) + STOP_BYTES));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, false, true, VT, const int2*>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(false, false) + STOP_BYTES));
+    MVSN_CUDA_CHECK(cudaFuncSetAttribute(render_wg_kernel<false, true, true, VT, const int2*>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(true, false) + STOP_BYTES));
     return MVSN_OK;
 }
 
@@ -942,10 +946,15 @@ template <typename VT>
 static void launch_wg_kernel(int grid, cudaStream_t stream, const SceneDev& sc, const RenderIO& io, const uint8_t* w, bool fast,
                              bool split, const float* t_stop, unsigned long long* tiles_done, const int2* ranges) {
     using namespace wg;
-    if (t_stop) {                                         // early ray termination: the ray entry only
+    if (t_stop) {                                         // early ray termination: the ray and the samples entries
         const int smem = smem_bytes(split, false) + STOP_BYTES, nthreads = threads(split, false);
-        if (split) render_wg_kernel<true, true, true, VT, const int2*><<<grid, nthreads, smem, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
-        else       render_wg_kernel<true, false, true, VT, const int2*><<<grid, nthreads, smem, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
+        if (fast) {
+            if (split) render_wg_kernel<true, true, true, VT, const int2*><<<grid, nthreads, smem, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
+            else       render_wg_kernel<true, false, true, VT, const int2*><<<grid, nthreads, smem, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
+        } else {
+            if (split) render_wg_kernel<false, true, true, VT, const int2*><<<grid, nthreads, smem, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
+            else       render_wg_kernel<false, false, true, VT, const int2*><<<grid, nthreads, smem, stream>>>(sc, io, w, *t_stop, tiles_done, ranges);
+        }
     } else if (split) {
         const int smem = smem_bytes(true, false), nthreads = threads(true, false);
         if (fast) render_wg_kernel<true, true, false, VT><<<grid, nthreads, smem, stream>>>(sc, io, w, 0.f, nullptr);

@@ -38,6 +38,7 @@ EXPORTS = [
     "mvsn_volume_to_half", "mvsn_costreg_forward_f16",
     "mvsn_occupancy_bytes", "mvsn_build_occupancy_workspace_bytes", "mvsn_build_occupancy",
     "mvsn_render_rays_occ_workspace_bytes", "mvsn_render_rays_occ",
+    "mvsn_render_samples_stop", "mvsn_render_backward_stop_workspace_bytes", "mvsn_render_backward_stop",
 ]
 VOLUME_F16 = 0x100       # OR-ed into RenderScene.mlp_mode (TC modes): volume_dhwc is an fp16 [D,Hp,Wp,8] image
 MAX_PEERS, PEER_HANDLE_BYTES = 16, 64
@@ -98,6 +99,7 @@ def load() -> C.CDLL:
     lib.mvsn_render_rays_stop.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), vp, vp, ip, ip, fp,
                                           vp, vp, vp, vp]
     lib.mvsn_render_rays_stop.restype = ip
+    lib.mvsn_render_samples_stop.argtypes = [C.POINTER(RenderScene), vp, vp, vp, vp, ip, ip, fp, vp, vp, vp, vp]
     for name in ("mvsn_occupancy_bytes", "mvsn_build_occupancy_workspace_bytes"):
         getattr(lib, name).restype = C.c_size_t
         getattr(lib, name).argtypes = [ip, ip, ip]
@@ -142,6 +144,10 @@ def load() -> C.CDLL:
     lib.mvsn_render_backward_rays_stop.argtypes = [C.POINTER(RenderScene), C.POINTER(vp), C.POINTER(RayParams), vp, vp,
                                                    vp, ip, ip, ip, ip, fp, C.POINTER(RenderGrads), C.POINTER(vp), vp,
                                                    vp, vp, vp, C.c_size_t, vp]
+    lib.mvsn_render_backward_stop_workspace_bytes.restype = C.c_size_t
+    lib.mvsn_render_backward_stop_workspace_bytes.argtypes = [ip, ip, ip, ip, ip, ip, ip]
+    lib.mvsn_render_backward_stop.argtypes = [C.POINTER(RenderScene), C.POINTER(vp), vp, vp, vp, vp, ip, ip, ip, ip, fp,
+                                              C.POINTER(RenderGrads), C.POINTER(vp), vp, vp, vp, vp, C.c_size_t, vp]
     lib.mvsn_adam_step.argtypes = [C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(ip), ip,
                                    fp, fp, fp, fp, ip, vp]
     lib.mvsn_adam_step_volume.argtypes = [vp, vp, vp, vp, C.c_longlong, ip, fp, fp, fp, fp, ip, vp]
@@ -159,7 +165,8 @@ def load() -> C.CDLL:
                  "mvsn_render_backward_deterministic", "mvsn_render_backward_rays",
                  "mvsn_render_backward_rays_stop", "mvsn_adam_step",
                  "mvsn_adam_step_volume", "mvsn_featurenet_forward_bn", "mvsn_costreg_forward_bn",
-                 "mvsn_volume_to_half", "mvsn_costreg_forward_f16", "mvsn_build_occupancy", "mvsn_render_rays_occ"):
+                 "mvsn_volume_to_half", "mvsn_costreg_forward_f16", "mvsn_build_occupancy", "mvsn_render_rays_occ",
+                 "mvsn_render_samples_stop", "mvsn_render_backward_stop"):
         getattr(lib, name).restype = ip
     _lib = lib
     return lib
