@@ -221,6 +221,42 @@ int mvsn_render_rays_occ(const mvsn_render_scene* scene, const mvsn_ray_params* 
                          const mvsn_occupancy* occupancy, float* rgb, float* depth, unsigned long long* tiles_done,
                          void* workspace, size_t workspace_bytes, void* stream);
 
+/* Importance sampling from a density grid (the reference's --use_density_volume --N_importance K).
+ *
+ * mvsn_build_density: sigma = relu(alpha_linear(h)) in fp32 at every node of the scene's D x Hp x Wp grid, laid out
+ * [D][Hp][Wp] (the shape of the reference's density_volume).  The nodes are mvsn_build_occupancy's (NDC = the node, the
+ * world point inverts utils.get_ndc_coordinate for rp), evaluated by the fp32 FFMA tile of MVSN_MLP_FP32.
+ * scene->mlp_mode must be MVSN_MLP_FP32 (| MVSN_VOLUME_F16: an fp16 volume image, whose grid equals the one of its fp32
+ * upcast bit for bit); scene->white_bkgd is unused; D, Hp, Wp >= 2.  sigma: D * Hp * Wp floats, 4-byte aligned,
+ * OVERWRITTEN.  Workspace: mvsn_build_density_workspace_bytes(D, Hp, Wp) bytes, 16-byte aligned (0 for a dim < 2).
+ * Argument errors are returned before any CUDA call.
+ *
+ * mvsn_sample_importance: data/ray_utils.ray_marcher_fine + sample_pdf for N rays [N,8] (16-byte aligned).  The S
+ * coarse depths come from one of two sources:
+ *   t_steps [S] (+ optional jitter [N,S]): marched from each ray's near / far as mvsn_render_backward_rays marches them,
+ *     their NDC by the render's get_ndc_coordinate (scene's reference camera, rp);  z_vals and ndc NULL;
+ *   z_vals [N,S] (nondecreasing or not) and ndc [N,S,3]: the caller's;  t_steps and jitter NULL.
+ * sigma_j is the grid's trilinear value at the sample's NDC (align_corners, zero padding; the NDC itself, not the
+ * reference's doubled 4 ndc - 3 mapping), alpha_j = 1 - exp(-relu(sigma_j)), w_j = alpha_j prod_{i<j}(1 - alpha_i + 1e-10),
+ * and K depths are drawn by inverse-CDF sampling of (w_1..w_{S-2} + 1e-5) over the midpoints of the coarse depths with
+ * u [N,K] (NULL: torch.linspace(0, 1, K) for every ray).  Outputs: z_out [N,S+K] = sort(cat(fine, coarse)) ascending
+ * (NaN last; the coarse values bit-exact), pts_out [N,S+K,3] = o + d * z (multiply, then add), ndc_out [N,S+K,3]
+ * (optional) their NDC.  scene and rp are needed by the march and ndc_out only (may be NULL otherwise); with a scene,
+ * the grid's dims must equal its volume's.  3 <= S, 1 <= K (MVSN_EBADSHAPE), S + K <= 1024 (MVSN_EUNSUPPORTED).
+ * Argument errors are returned before any CUDA call. */
+typedef struct mvsn_density {
+    const float* sigma;         /* device [D][Hp][Wp] fp32, 4-byte aligned */
+    int D, Hp, Wp;
+} mvsn_density;
+
+size_t mvsn_build_density_workspace_bytes(int D, int Hp, int Wp);
+int mvsn_build_density(const mvsn_render_scene* scene, const mvsn_ray_params* rp, float* sigma, void* workspace,
+                       size_t workspace_bytes, void* stream);
+int mvsn_sample_importance(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const mvsn_density* density,
+                           const float* rays, const float* t_steps, const float* jitter, const float* z_vals,
+                           const float* ndc, const float* u, int N, int S, int K, float* z_out, float* pts_out,
+                           float* ndc_out, void* stream);
+
 /* Ray generation for one camera (replaces: data/ray_utils.get_rays, data/ray_utils.py:32-53, and the notebooks'
  * `torch.cat([rays_o, rays_d, near, far])`): directions [n,3] = get_ray_directions(H, W, focal) in camera coordinates
  * (resident on the device, they depend on the intrinsics only), c2w = the first three rows of the camera-to-world matrix,

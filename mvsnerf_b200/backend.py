@@ -452,10 +452,10 @@ def _images_packed(imgs):
     return _cached("imgs", imgs, build), (V, H, W)
 
 
-def _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode, half_ok=False):
+def _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode, half_ok=False, half_fp32=False):
     """half_ok: a forward render that may read a float16 volume as fp16 (tensor-core modes only); otherwise a half
-    volume is upcast to a cached fp32 image."""
-    vol, (D, Hp, Wp) = _volume_channels_last(volume_feature, half_ok and mode != _lib.MLP_FP32)
+    volume is upcast to a cached fp32 image.  half_fp32: MLP_FP32 reads it as fp16 too (mvsn_build_density)."""
+    vol, (D, Hp, Wp) = _volume_channels_last(volume_feature, half_ok and (mode != _lib.MLP_FP32 or half_fp32))
     im, (V, H, W) = _images_packed(imgs)
     if V != 3:
         raise RuntimeError(f"{V} source views: the v0 network takes exactly 3 (feat_dim = 8 + 3*4)")
@@ -1001,15 +1001,39 @@ class FineTuner:
         return self.loss, (rgb, depth)
 
     def step_rays(self, rays, target_rgb, near_far, pad, N_samples=128, lindisp=False, perturb=1.0, generator=None,
-                  lr=None, want_forward=False, t_stop=None):
+                  lr=None, want_forward=False, t_stop=None, density=None, N_importance=0):
         """One optimisation step on a batch of rays [N,8] = (o, d, near, far), as train_mvs_nerf_finetuning_pl.py:140-164
         feeds it: the ray march (ray_marcher with `perturb`) and the NDC conversion run inside the backward kernel
         (render_backward_rays).  With perturb > 0 the jitter is drawn as ray_marcher draws it, `perturb *
         torch.rand((N, N_samples))` (from `generator`, or the default generator), so switching a run from
         `step(*ray_marcher(...))` to step_rays consumes the same random stream.  `near_far` / `pad` as in render_rays.
         `t_stop`: early ray termination, as in render_backward_rays -- the step trains the render truncated where each
-        ray's transmittance falls below t_stop, and skips the work of the samples behind.  Returns what `step` returns."""
+        ray's transmittance falls below t_stop, and skips the work of the samples behind.  Returns what `step` returns.
+
+        `density` (a `Density` from build_density, or a CUDA fp32 sigma tensor [D, Hp, Wp]) with `N_importance` = K >= 1:
+        the reference's --use_density_volume --N_importance K step (train_mvs_nerf_finetuning_pl.py:150-164).  The
+        jitter [N, N_samples] and then u [N, K] are drawn from `generator` in the reference's order (ray_marcher, then
+        sample_pdf); mvsn_sample_importance marches the jittered coarse samples, draws K more from the grid and sorts
+        them; the step is then `step` on those N_samples + K samples (render_backward).  N_samples + K <= 128 (the
+        backward's limit) and grad_mode MLP_FP32 or MLP_TC_HALF: otherwise RuntimeError before any launch."""
         lr = self.lr if lr is None else float(lr)
+        if density is not None or N_importance:
+            S, K = _importance_shape(N_samples, N_importance, "FineTuner.step_rays", max_total=128)
+            if density is None:
+                raise RuntimeError("FineTuner.step_rays: N_importance needs density= (a Density from build_density)")
+            if self.grad_mode == _lib.GRAD_TC_FULL:
+                raise RuntimeError("FineTuner.step_rays: importance sampling trains through the samples entries, which "
+                                   "run MLP_FP32 or MLP_TC_HALF (grad_mode GRAD_TC_FULL given)")
+            sigma = _density_sigma(density, "FineTuner.step_rays", near_far, pad, lindisp)
+            rays = _lib.dev_f32(rays.detach(), "rays")
+            n = rays.shape[0]
+            jitter = None
+            if perturb > 0:
+                jitter = perturb * torch.rand((n, S), device=rays.device, generator=generator)
+            u = torch.rand((n, K), device=rays.device, generator=generator)
+            z, pts, ndc = sample_importance(rays, sigma, self.volume, self.imgs, self.pose_ref, self.network_fn, near_far,
+                                            pad, N_samples=S, N_importance=K, lindisp=lindisp, jitter=jitter, u=u)
+            return self.step(pts, ndc, z, rays[:, 3:6], target_rgb, lr=lr, want_forward=want_forward, t_stop=t_stop)
         rays = _lib.dev_f32(rays.detach(), "rays")
         jitter = None
         if perturb > 0:
@@ -1240,9 +1264,223 @@ def build_occupancy(volume_feature, imgs, pose_ref, network_fn, near_far, pad, l
     return occ
 
 
+# --------------------------------------------------------------------------------------------
+# importance sampling from a density grid (data/ray_utils.py:98-141 sample_pdf, :199-224 ray_marcher_fine)
+# --------------------------------------------------------------------------------------------
+IMPORTANCE_CHUNK_RAYS = 32768   # rays per sampler + render launch pair in render_rays (a multiple of 32)
+_imp_buffers = {}               # per device: z / pts / ndc / dirs of one chunk, grown to the largest
+
+
+class Density:
+    """A density grid of a scene for importance sampling: sigma [D, Hp, Wp] (fp32, the reference's density_volume
+    layout) at the encoding volume's nodes in NDC, and the geometry it was built for -- the rays' NDC mapping must be
+    the same (near_far, pad, lindisp) for it to apply."""
+
+    def __init__(self, sigma, near_far, pad, lindisp):
+        self.sigma = sigma
+        self.D, self.Hp, self.Wp = (int(v) for v in sigma.shape)
+        self.near_far, self.pad, self.lindisp = (float(near_far[0]), float(near_far[1])), float(pad), bool(lindisp)
+
+
+def build_density(volume_feature, imgs, pose_ref, network_fn, near_far, pad, lindisp=False):
+    """The density grid of a scene (mvsn_build_density): sigma = relu(alpha_linear(h)) at every node of the volume's
+    grid, the node as the sample's NDC and the world point from inverting get_ndc_coordinate with `near_far` / `pad` /
+    `lindisp` (the nodes of build_occupancy), evaluated in fp32 by the FFMA tile.  fp32 and fp16 volumes (an fp16
+    volume gives the grid of its fp32 upcast, bit for bit).  Returns a `Density`.
+
+    This is the reference's update_density_volume (train_mvs_nerf_finetuning_pl.py:91-99) with sigma taken where the
+    renderer evaluates it: at the node's NDC, not at its positionally encoded world point (DESIGN §5).  The grid is
+    cached on the version counters of the volume, the MLP, the images and cameras, as build_occupancy's: FineTuner's
+    Adam step bumps them, so calling build_density every 200 steps rebuilds it after an update."""
+    owner = volume_feature.feat_volume if isinstance(volume_feature, nn.Module) else volume_feature
+    if not owner.is_cuda:
+        raise RuntimeError("build_density: the encoding volume must be a CUDA tensor; mvsnerf_b200 has no CPU path")
+    params = network_fn.ordered_params()
+    tensors = [owner, imgs, pose_ref["w2cs"], pose_ref["intrinsics"]] + list(params)
+    args = (float(near_far[0]), float(near_far[1]), float(pad), bool(lindisp))
+    hit = _cache.get("density")
+    if hit is not None and hit[1] == args and len(hit[0]) == len(tensors) and \
+            all(r() is t and v == t._version for (r, v), t in zip(hit[0], tensors)):
+        cache_stats["hit"] += 1
+        return hit[2]
+    cache_stats["miss"] += 1
+    lib = _lib.load()
+    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, False, _lib.MLP_FP32, half_ok=True, half_fp32=True)
+    dev = owner.device
+    rp = _lib.RayParams(args[0], args[1], args[2], int(args[3]))
+    need = lib.mvsn_build_density_workspace_bytes(sc.D, sc.Hp, sc.Wp)
+    if need == 0:
+        raise RuntimeError(f"build_density: volume {sc.D}x{sc.Hp}x{sc.Wp} (every dim >= 2)")
+    sigma = torch.empty(sc.D, sc.Hp, sc.Wp, dtype=torch.float32, device=dev)
+    ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.mvsn_build_density(C.byref(sc), C.byref(rp), _lib.ptr(sigma), _lib.ptr(ws), need,
+                                          _lib.stream_ptr()), "mvsn_build_density")
+    del keep
+    den = Density(sigma, near_far, pad, lindisp)
+    _cache["density"] = ([(weakref.ref(t), t._version) for t in tensors], args, den)
+    return den
+
+
+def _importance_shape(N_samples, N_importance, who, max_total=1024):
+    """(S, K) after the sampler's limits: 3 <= S, 1 <= K, S + K <= max_total"""
+    S, K = int(N_samples), int(N_importance)
+    if S < 3 or K < 1:
+        raise RuntimeError(f"{who}: N_samples={S}, N_importance={K} (importance sampling needs N_samples >= 3 and "
+                           "N_importance >= 1)")
+    if S + K > max_total:
+        raise RuntimeError(f"{who}: N_samples + N_importance = {S + K} exceeds {max_total}"
+                           + (" (the fine-tuning backward's N_samples limit)" if max_total == 128 else ""))
+    return S, K
+
+
+def _density_sigma(density, who, near_far=None, pad=None, lindisp=None):
+    """The sigma tensor of a `Density` (checked against the rays' geometry when it is given) or of a CUDA fp32 [D,H,W]
+    tensor (the reference's density_volume)."""
+    if isinstance(density, Density):
+        if near_far is not None and (density.near_far != (float(near_far[0]), float(near_far[1])) or
+                                     density.pad != float(pad) or density.lindisp != bool(lindisp)):
+            raise RuntimeError(f"{who}: the density grid was built for another near_far / pad / lindisp")
+        return density.sigma
+    if isinstance(density, torch.Tensor) and density.is_cuda and density.dtype == torch.float32 and density.dim() == 3:
+        return density.detach().contiguous()
+    raise RuntimeError(f"{who}: density must be a Density from build_density or a CUDA fp32 tensor [D, H, W]")
+
+
+def _sample_importance_launch(sc, rp, sigma, rays, t_steps, jitter, z_vals, ndc_in, u, N, S, K, z, pts, ndc):
+    grid = _lib.DensityGrid(sigma.data_ptr(), *[int(v) for v in sigma.shape])
+    _lib.check(_lib.load().mvsn_sample_importance(
+        None if sc is None else C.byref(sc), None if rp is None else C.byref(rp), C.byref(grid), _lib.ptr(rays),
+        _lib.ptr(t_steps), _lib.ptr(jitter), _lib.ptr(z_vals), _lib.ptr(ndc_in), _lib.ptr(u), int(N), int(S), int(K),
+        _lib.ptr(z), _lib.ptr(pts), _lib.ptr(ndc), _lib.stream_ptr()), "mvsn_sample_importance")
+
+
+def _opt_draws(t, n, k, name, who):
+    if t is None:
+        return None
+    t = _lib.dev_f32(t.detach(), name)
+    if tuple(t.shape) != (n, k):
+        raise RuntimeError(f"{who}: {name} must be [{n}, {k}], got {tuple(t.shape)}")
+    return t
+
+
+def sample_importance(rays, density, volume_feature, imgs, pose_ref, network_fn, near_far, pad, N_samples=64,
+                      N_importance=64, lindisp=False, jitter=None, u=None):
+    """The importance sampler on rays [N,8] (mvsn_sample_importance, marched source): ray_marcher with `N_samples`,
+    `lindisp` and the stratification `jitter` [N, N_samples] (= perturb * u as ray_marcher draws it; None: none),
+    then ray_marcher_fine's K = `N_importance` samples from `density` with the uniform draws `u` [N, K] (None:
+    torch.linspace(0, 1, K)).  Returns (z [N,S+K] sorted, pts [N,S+K,3] = o + d z, ndc [N,S+K,3]): the samples
+    `rendering` / `FineTuner.step` take, the NDC by the render's get_ndc_coordinate for `near_far` / `pad`."""
+    S, K = _importance_shape(N_samples, N_importance, "sample_importance")
+    sigma = _density_sigma(density, "sample_importance", near_far, pad, lindisp)
+    rays = _lib.dev_f32(rays.detach(), "rays")
+    n, dev = rays.shape[0], rays.device
+    jitter = _opt_draws(jitter, n, S, "jitter", "sample_importance")
+    u = _opt_draws(u, n, K, "u", "sample_importance")
+    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, False, _lib.MLP_FP32)
+    rp = _lib.RayParams(float(near_far[0]), float(near_far[1]), float(pad), int(bool(lindisp)))
+    z = torch.empty(n, S + K, dtype=torch.float32, device=dev)
+    pts = torch.empty(n, S + K, 3, dtype=torch.float32, device=dev)
+    ndc = torch.empty(n, S + K, 3, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _sample_importance_launch(sc, rp, sigma, rays, _tsteps_of(S, dev), jitter, None, None, u, n, S, K, z, pts, ndc)
+    del keep
+    return z, pts, ndc
+
+
+def ray_marcher_fine(rays, density_volume, z_vals, pts_NDC, N_importance=64, lindisp=False):
+    """data/ray_utils.py:199-224 on the GPU (mvsn_sample_importance, the caller's coarse samples): K = N_importance
+    depths per ray drawn by inverse-CDF sampling of the density grid's weights along z_vals [N,S] (looked up at
+    pts_NDC [N,S,3]), merged with z_vals and sorted.  Returns (xyz [N,S+K,3], rays_o, rays_d, z_vals [N,S+K]), as the
+    reference does; the caller recomputes the NDC.  `density_volume`: a `Density` or a CUDA fp32 tensor [D,H,W].  u is
+    drawn as sample_pdf draws it, torch.rand((N, K)) from the default generator on the rays' device, so a seeded run
+    consumes the same stream.  The grid is looked up at pts_NDC itself, the volume's own mapping, where the reference
+    maps the coordinate twice (DESIGN §5).  `lindisp` is accepted and unused, as in the reference."""
+    n, S = int(z_vals.shape[0]), int(z_vals.shape[1])
+    S, K = _importance_shape(S, N_importance, "ray_marcher_fine")
+    sigma = _density_sigma(density_volume, "ray_marcher_fine")
+    r = _lib.dev_f32(rays.detach(), "rays")
+    z_in = _lib.dev_f32(z_vals.detach(), "z_vals")
+    ndc_in = _lib.dev_f32(pts_NDC.detach(), "pts_NDC")
+    if tuple(ndc_in.shape) != (n, S, 3) or r.shape[0] != n:
+        raise RuntimeError(f"ray_marcher_fine: rays [{n},8], z_vals [{n},{S}] and pts_NDC [{n},{S},3] expected, got "
+                           f"{tuple(r.shape)}, {tuple(z_vals.shape)} and {tuple(pts_NDC.shape)}")
+    dev = r.device
+    u = torch.rand((n, K), device=rays.device)
+    z = torch.empty(n, S + K, dtype=torch.float32, device=dev)
+    xyz = torch.empty(n, S + K, 3, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _sample_importance_launch(None, None, sigma, r, None, None, z_in, ndc_in, u, n, S, K, z, xyz, None)
+    return xyz, rays[:, 0:3], rays[:, 3:6], z
+
+
+def render_density(network_fn, rays_pts, density_feature, network_query_fn, chunk=1024 * 5):
+    """renderer.render_density (renderer.py:167-177), unchanged: network_query_fn(pts, None, feats, network_fn) over
+    chunks of `chunk` points, concatenated -- what an unchanged update_density_volume calls.  build_density computes the
+    grid in one launch instead."""
+    densities = []
+    device = density_feature.device
+    for i in range(0, rays_pts.shape[0], chunk):
+        densities.append(network_query_fn(rays_pts[i:i + chunk].to(device), None, density_feature[i:i + chunk],
+                                          network_fn))
+    return torch.cat(densities)
+
+
+def _render_rays_importance(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad, N_samples, white_bkgd,
+                            lindisp, mode, out, t_stop, tiles_done, density, N_importance, importance_u):
+    """render_rays(density=, N_importance=): per chunk of IMPORTANCE_CHUNK_RAYS rays, mvsn_sample_importance (linspace
+    coarse samples, their NDC) then mvsn_render_samples[_stop] on the S + K samples."""
+    if density is None:
+        raise RuntimeError("render_rays: N_importance needs density= (a Density from build_density)")
+    S, K = _importance_shape(N_samples, N_importance, "render_rays")
+    sigma = _density_sigma(density, "render_rays", near_far, pad, lindisp)
+    if t_stop is not None:
+        t_stop = float(t_stop)
+        if not t_stop >= 0.0:
+            raise RuntimeError(f"render_rays: t_stop={t_stop} must be >= 0")
+        _check_counter(tiles_done, "render_rays", "tiles_done", torch.int64, 1, rays.device)
+    lib = _lib.load()
+    rays = _lib.dev_f32(rays, "rays")
+    N, dev, M = rays.shape[0], rays.device, S + K
+    u = _opt_draws(importance_u, N, K, "importance_u", "render_rays")
+    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, mode, half_ok=True)
+    rp = _lib.RayParams(float(near_far[0]), float(near_far[1]), float(pad), int(bool(lindisp)))
+    if out is not None:
+        rgb, depth = out
+    else:
+        rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
+        depth = torch.empty(N, dtype=torch.float32, device=dev)
+    chunk = max(1, min(N, IMPORTANCE_CHUNK_RAYS))
+    buf = _imp_buffers.get(dev)
+    if buf is None or buf.numel() < chunk * M * 7 + chunk * 3:
+        buf = torch.empty(chunk * M * 7 + chunk * 3, dtype=torch.float32, device=dev)
+        _imp_buffers[dev] = buf
+    t_steps = _tsteps_of(S, dev)
+    with torch.cuda.device(dev):
+        for c0 in range(0, N, chunk):
+            n = min(chunk, N - c0)
+            r = rays[c0:c0 + n]
+            z, pts, ndc = buf[:n * M], buf[n * M:4 * n * M], buf[4 * n * M:7 * n * M]
+            dirs = buf[7 * n * M:7 * n * M + 3 * n].view(n, 3)
+            dirs.copy_(r[:, 3:6])
+            _sample_importance_launch(sc, rp, sigma, r, t_steps, None, None, None, None if u is None else u[c0:c0 + n],
+                                      n, S, K, z, pts, ndc)
+            if t_stop is None:
+                _lib.check(lib.mvsn_render_samples(C.byref(sc), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z), _lib.ptr(dirs),
+                                                   n, M, _lib.ptr(rgb[c0:c0 + n]), _lib.ptr(depth[c0:c0 + n]), None,
+                                                   None, None, _lib.stream_ptr()), "mvsn_render_samples")
+            else:
+                _lib.check(lib.mvsn_render_samples_stop(C.byref(sc), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z),
+                                                        _lib.ptr(dirs), n, M, t_stop, _lib.ptr(rgb[c0:c0 + n]),
+                                                        _lib.ptr(depth[c0:c0 + n]), _lib.ptr(tiles_done),
+                                                        _lib.stream_ptr()), "mvsn_render_samples_stop")
+    del keep
+    return rgb, depth
+
+
 def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad, N_samples=128,
                 white_bkgd=False, lindisp=False, mlp_mode=None, out=None, sink=None, t_stop=None, tiles_done=None,
-                occupancy=None):
+                occupancy=None, density=None, N_importance=0, importance_u=None):
     """Fused-caller entry: one launch renders all `rays` [N,8] = (o, d, near, far).
 
     Replaces the notebooks' per-chunk loop `ray_marcher -> get_ndc_coordinate -> rendering`
@@ -1268,9 +1506,27 @@ def render_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad,
 
     A float16 `volume_feature` is read as fp16 in the tensor-core modes (half the resident bytes): the result is
     bit-identical to rendering `volume.float()`.  Channels-last storage (MVSNet.forward(..., volume_dtype=torch.float16),
-    or `.half()` of an fp32 MVSNet volume) is read in place; other layouts are converted once per tensor version."""
+    or `.half()` of an fp32 MVSNet volume) is read in place; other layouts are converted once per tensor version.
+
+    `density` (a `Density` from build_density for this near_far / pad / lindisp, or a CUDA fp32 sigma tensor
+    [D, Hp, Wp]) with `N_importance` = K >= 1: importance sampling (the reference's --use_density_volume --N_importance).
+    Each ray's N_samples linspace samples and K more drawn from the grid by inverse-CDF sampling (mvsn_sample_importance),
+    sorted, are rendered by the samples entry (mvsn_render_samples, or mvsn_render_samples_stop with t_stop) in any
+    mlp_mode, in chunks of IMPORTANCE_CHUNK_RAYS rays.  `importance_u` [N, K]: the uniform draws (the reference's
+    validation draws torch.rand); None draws torch.linspace(0, 1, K) for every ray, a reproducible frame.  Not
+    combinable with `occupancy` or `sink`."""
     lib = _lib.load()
     mode = DEFAULT_MLP_MODE if mlp_mode is None else mlp_mode
+    if density is not None or N_importance or importance_u is not None:
+        if occupancy is not None or sink is not None:
+            raise RuntimeError("render_rays: density (importance sampling) cannot be combined with occupancy or sink")
+        if t_stop is not None and mode == _lib.MLP_FP32:
+            raise RuntimeError("render_rays: t_stop needs a tensor-core mlp_mode (MLP_TC_HALF / TC_PAIR / TC_SPLIT)")
+        if t_stop is None and tiles_done is not None:
+            raise RuntimeError("render_rays: tiles_done needs t_stop")
+        return _render_rays_importance(rays, volume_feature, imgs, pose_ref, network_fn, near_far, pad, N_samples,
+                                       white_bkgd, lindisp, mode, out, t_stop, tiles_done, density, N_importance,
+                                       importance_u)
     if occupancy is not None:
         if sink is not None:
             raise RuntimeError("render_rays: occupancy cannot be combined with sink (peer frame assembly)")
@@ -1435,7 +1691,8 @@ def _network_query(pts, viewdirs, rays_feats, network_fn, netchunk=1024):
 
 def create_nerf_mvs(args, pts_embedder=True, use_mvs=False, dir_embedder=True, device=None):
     """Same contract as models.create_nerf_mvs: returns
-    (render_kwargs_train, render_kwargs_test, start, grad_vars).  When `args` has a `t_stop` attribute that is not
+    (render_kwargs_train, render_kwargs_test, start, grad_vars).  N_importance > 0 creates `network_fine` as the
+    reference does (an MLP `rendering` ignores; its parameters join grad_vars).  When `args` has a `t_stop` attribute that is not
     None, both kwargs dicts also carry it, so `rendering(args, ..., **render_kwargs)` runs with early ray termination
     (see rendering); otherwise the dicts are exactly the reference's."""
     if not pts_embedder or dir_embedder:
@@ -1448,8 +1705,13 @@ def create_nerf_mvs(args, pts_embedder=True, use_mvs=False, dir_embedder=True, d
     model = MVSNeRF(D=args.netdepth, W=args.netwidth, input_ch_pts=args.pts_dim * (1 + 2 * args.multires),
                     input_ch_views=args.dir_dim, input_ch_feat=args.feat_dim, net_type=args.net_type).to(device)
     grad_vars = list(model.parameters())
+    model_fine = None
     if getattr(args, "N_importance", 0) > 0:
-        raise RuntimeError("N_importance > 0 (hierarchical sampling) is outside the hot path (SURVEY.md 2.1)")
+        # models.py:593-598: a second MLP whose parameters join grad_vars; `rendering` never runs it (nor does the
+        # reference's), the importance samples are drawn from the density grid (build_density / ray_marcher_fine)
+        model_fine = MVSNeRF(D=args.netdepth, W=args.netwidth, input_ch_pts=args.pts_dim * (1 + 2 * args.multires),
+                             input_ch_views=args.dir_dim, input_ch_feat=args.feat_dim).to(device)
+        grad_vars += list(model_fine.parameters())
     encoding_net = None
     if use_mvs:
         encoding_net = MVSNet().to(device)
@@ -1464,7 +1726,7 @@ def create_nerf_mvs(args, pts_embedder=True, use_mvs=False, dir_embedder=True, d
     render_kwargs_train = {
         "network_query_fn": lambda pts, viewdirs, rays_feats, network_fn: _network_query(
             pts, viewdirs, rays_feats, network_fn, args.netchunk),
-        "perturb": args.perturb, "N_importance": args.N_importance, "network_fine": None,
+        "perturb": args.perturb, "N_importance": args.N_importance, "network_fine": model_fine,
         "N_samples": args.N_samples, "network_fn": model, "network_mvs": encoding_net,
         "use_viewdirs": args.use_viewdirs, "white_bkgd": args.white_bkgd, "raw_noise_std": args.raw_noise_std,
     }

@@ -428,6 +428,69 @@ int mvsn_build_occupancy(const mvsn_render_scene* scene, const mvsn_ray_params* 
                            (cudaStream_t)stream);
 }
 
+size_t mvsn_build_density_workspace_bytes(int D, int Hp, int Wp) { return density_workspace_bytes(D, Hp, Wp); }
+
+int mvsn_build_density(const mvsn_render_scene* scene, const mvsn_ray_params* rp, float* sigma, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_build_density");
+    SceneDev sc;
+    int rc = make_scene(scene, sc);
+    if (rc) return rc;
+    MVSN_REQUIRE(rp && sigma && workspace, MVSN_ENULL, "mvsn_build_density: NULL argument");
+    MVSN_REQUIRE(mlp_mode_of(scene) == MVSN_MLP_FP32, MVSN_EUNSUPPORTED,
+                 "mvsn_build_density: scene->mlp_mode %d (the MVSN_MLP_FP32 image, optionally | MVSN_VOLUME_F16)",
+                 scene->mlp_mode);
+    MVSN_REQUIRE(scene->D >= 2 && scene->Hp >= 2 && scene->Wp >= 2, MVSN_EBADSHAPE,
+                 "mvsn_build_density: volume %dx%dx%d (every dim >= 2)", scene->D, scene->Hp, scene->Wp);
+    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(sigma) % 4 == 0, MVSN_EALIGN, "mvsn_build_density: sigma must be 4-byte aligned");
+    MVSN_REQUIRE(aligned16(workspace), MVSN_EALIGN, "mvsn_build_density: workspace must be 16-byte aligned");
+    const size_t need = density_workspace_bytes(scene->D, scene->Hp, scene->Wp);
+    MVSN_REQUIRE(workspace_bytes >= need, MVSN_EWORKSPACE, "mvsn_build_density: workspace needs %zu bytes, got %zu", need,
+                 workspace_bytes);
+    return build_density(sc, make_ray_gen(scene, rp), static_cast<const float*>(scene->mlp_packed), half_volume(scene),
+                         sigma, workspace, (cudaStream_t)stream);
+}
+
+int mvsn_sample_importance(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const mvsn_density* density,
+                           const float* rays, const float* t_steps, const float* jitter, const float* z_vals,
+                           const float* ndc, const float* u, int N, int S, int K, float* z_out, float* pts_out,
+                           float* ndc_out, void* stream) {
+    MVSN_RANGE("mvsn_sample_importance");
+    const char* what = "mvsn_sample_importance";
+    MVSN_REQUIRE(N >= 0 && S >= 3 && K >= 1, MVSN_EBADSHAPE, "%s: N=%d S=%d K=%d (S >= 3, K >= 1)", what, N, S, K);
+    MVSN_REQUIRE(S + K <= MAX_IMPORTANCE_SAMPLES, MVSN_EUNSUPPORTED, "%s: S + K = %d (at most %d)", what, S + K,
+                 MAX_IMPORTANCE_SAMPLES);
+    MVSN_REQUIRE(density && density->sigma && rays && z_out && pts_out, MVSN_ENULL, "%s: NULL required pointer", what);
+    MVSN_REQUIRE((t_steps != nullptr) != (z_vals != nullptr), MVSN_ENULL,
+                 "%s: exactly one coarse source: t_steps (marched) or z_vals + ndc", what);
+    MVSN_REQUIRE(t_steps || ndc, MVSN_ENULL, "%s: z_vals needs ndc", what);
+    MVSN_REQUIRE(!z_vals || !jitter, MVSN_EUNSUPPORTED, "%s: jitter applies to the marched source only", what);
+    const bool cams = t_steps != nullptr || ndc_out != nullptr;
+    MVSN_REQUIRE(!cams || (scene && rp), MVSN_ENULL, "%s: the march and ndc_out need scene and rp", what);
+    SceneDev sc{};
+    if (scene) {
+        int rc = make_scene(scene, sc);
+        if (rc) return rc;
+    }
+    MVSN_REQUIRE(aligned16(rays), MVSN_EALIGN, "%s: rays must be 16-byte aligned", what);
+    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(density->sigma) % 4 == 0, MVSN_EALIGN, "%s: density->sigma must be 4-byte aligned",
+                 what);
+    MVSN_REQUIRE(density->D >= 2 && density->Hp >= 2 && density->Wp >= 2, MVSN_EBADSHAPE,
+                 "%s: density grid %dx%dx%d (every dim >= 2)", what, density->D, density->Hp, density->Wp);
+    MVSN_REQUIRE(!scene || (density->D == scene->D && density->Hp == scene->Hp && density->Wp == scene->Wp), MVSN_EBADSHAPE,
+                 "%s: density grid %dx%dx%d does not match the scene's volume %dx%dx%d", what, density->D, density->Hp,
+                 density->Wp, scene ? scene->D : 0, scene ? scene->Hp : 0, scene ? scene->Wp : 0);
+    if (N == 0) return MVSN_OK;
+    sc.D = density->D; sc.Hp = density->Hp; sc.Wp = density->Wp;
+    ImportanceIO io{};
+    io.rays = rays; io.t_steps = t_steps; io.jitter = jitter; io.z_in = z_vals; io.ndc_in = ndc;
+    io.sigma = density->sigma; io.u = u;
+    io.N = N; io.S = S; io.K = K; io.cams = cams;
+    io.z_out = z_out; io.pts_out = pts_out; io.ndc_out = ndc_out;
+    const RayGenDev rg = cams ? make_ray_gen(scene, rp) : RayGenDev{};
+    return launch_importance(sc, rg, io, (cudaStream_t)stream);
+}
+
 int mvsn_render_rays_to_peers(const mvsn_render_scene* scene, const mvsn_ray_params* rp, const float* rays,
                               const float* t_steps, int N, int S, const mvsn_peer_sink* sink, float* rgb,
                               float* depth, void* stream) {

@@ -7,7 +7,11 @@
 // eight corner nodes, sigma evaluated by the split-mode samples entry with the node as the sample's NDC, then dilated by
 // a (2 dilate + 1)^3 box.  sigma depends on the position only (the view direction enters the colour head alone), so a
 // grid serves every view of the scene.
-#include "render_frontend.cuh"
+//
+// Density grid (mvsn_build_density, the importance sampler's input): sigma itself, fp32, at every node, laid out
+// [D][Hp][Wp] -- the same node samples, evaluated by the fp32 forward tile (tile_fp32.cuh) that the FFMA render and the
+// fine-tuning backward share, which leaves sigma = relu(alpha_linear(h)) before any exponential.
+#include "tile_fp32.cuh"
 
 namespace mvsn {
 
@@ -165,6 +169,78 @@ int build_occupancy(const SceneDev& sc, const RayGenDev& rg, const void* wimg_sp
     }
     occ_pack_kernel<<<grid_of(n), 256, 0, stream>>>(cur, n, bits);
     MVSN_CUDA_CHECK(cudaGetLastError());
+    return MVSN_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// density grid
+// ------------------------------------------------------------------------------------------------
+// sigma of the io.N x io.S node samples occ_nodes_kernel wrote (sample i = ray i / S, step i % S): 128 consecutive
+// samples per tile, tiles strided over the CTAs.  VT = __half: sc.vol is the fp16 image (sample_volume<__half>), so the
+// grid equals the one of the volume vol.half().float() bit for bit.
+template <typename VT>
+__global__ void __launch_bounds__(256, 1) density_tile_kernel(const SceneDev sc, const RenderIO io,
+                                                               const float* __restrict__ wts, float* __restrict__ sigma) {
+    extern __shared__ __align__(16) float smem[];
+    const TileSmem sm(smem);
+    const int tid = threadIdx.x;
+    __shared__ Cams cams;
+    load_cams(sc, &cams, tid);
+    __syncthreads();
+    const long long n = (long long)io.N * io.S, ntiles = (n + TILE_M - 1) / TILE_M;
+    for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const long long i = t * TILE_M + tid;
+        const bool valid = tid < TILE_M && i < n;
+        if (tid < TILE_M)
+            tile_front_end<false, NoRecord, VT>(sc, cams, io, sm, tid, valid ? (int)(i / io.S) : 0,
+                                                valid ? (int)(i % io.S) : 0, valid, NoRecord{});
+        __syncthreads();
+        tile_mlp(sm, wts, tid, NoRecord{});
+        if (valid) sigma[i] = sm.sig[tid];                     // written by this thread inside tile_mlp
+        __syncthreads();
+    }
+}
+
+// workspace: one chunk of node samples, laid out as build_occupancy's
+size_t density_workspace_bytes(int D, int Hp, int Wp) {
+    if (D < 2 || Hp < 2 || Wp < 2) return 0;
+    const size_t cs = (size_t)occ::chunk_rows(D, Hp, Wp) * Wp;
+    return 2 * occ::round16(cs * 12) + occ::round16(cs * 4) + occ::round16((size_t)occ::chunk_rows(D, Hp, Wp) * 12);
+}
+
+int build_density(const SceneDev& sc, const RayGenDev& rg, const float* wts_fp32, bool half_vol, float* sigma,
+                  void* workspace, cudaStream_t stream) {
+    constexpr int SMEM = TILE_SMEM_FLOATS * sizeof(float);
+    static bool attr_set[64] = {false};                   // once per device, not per launch
+    int dev = 0;
+    MVSN_CUDA_CHECK(cudaGetDevice(&dev));
+    if (dev >= 64 || !attr_set[dev]) {
+        MVSN_CUDA_CHECK(cudaFuncSetAttribute(density_tile_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+        MVSN_CUDA_CHECK(cudaFuncSetAttribute(density_tile_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+        if (dev < 64) attr_set[dev] = true;
+    }
+    const int D = sc.D, Hp = sc.Hp, Wp = sc.Wp;
+    const int R = occ::chunk_rows(D, Hp, Wp);
+    const size_t cs = (size_t)R * Wp;
+    uint8_t* p = static_cast<uint8_t*>(workspace);
+    float* pts = reinterpret_cast<float*>(p);                   p += occ::round16(cs * 12);
+    float* ndc = reinterpret_cast<float*>(p);                   p += occ::round16(cs * 12);
+    float* z = reinterpret_cast<float*>(p);                     p += occ::round16(cs * 4);
+    float* dirs = reinterpret_cast<float*>(p);
+    for (int row0 = 0; row0 < D * Hp; row0 += R) {
+        const int rows = D * Hp - row0 < R ? D * Hp - row0 : R;
+        occ_nodes_kernel<<<grid_of((long long)rows * Wp), 256, 0, stream>>>(sc, rg, row0, rows, pts, ndc, z, dirs);
+        MVSN_CUDA_CHECK(cudaGetLastError());
+        RenderIO io{};
+        io.pts = pts; io.ndc = ndc; io.z = z; io.dirs = dirs;
+        io.N = rows; io.S = Wp;
+        const long long tiles = ((long long)rows * Wp + TILE_M - 1) / TILE_M;
+        const int grid = tiles < sm_count() ? (int)tiles : sm_count();
+        float* out = sigma + (size_t)row0 * Wp;
+        if (half_vol) density_tile_kernel<__half><<<grid, 256, SMEM, stream>>>(sc, io, wts_fp32, out);
+        else          density_tile_kernel<float><<<grid, 256, SMEM, stream>>>(sc, io, wts_fp32, out);
+        MVSN_CUDA_CHECK(cudaGetLastError());
+    }
     return MVSN_OK;
 }
 

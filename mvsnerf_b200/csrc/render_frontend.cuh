@@ -82,6 +82,22 @@ int build_occupancy(const SceneDev& sc, const RayGenDev& rg, const void* wimg_sp
                     uint32_t* bits, void* workspace, cudaStream_t stream);
 int launch_occupancy_ranges(const SceneDev& sc, const RenderIO& io, bool precise, const uint32_t* bits, int2* ranges,
                             cudaStream_t stream);
+// occupancy.cu: the density grid (mvsn_build_density): fp32 sigma [D][Hp][Wp] at the nodes, by the fp32 forward tile
+size_t density_workspace_bytes(int D, int Hp, int Wp);
+int build_density(const SceneDev& sc, const RayGenDev& rg, const float* wts_fp32, bool half_vol, float* sigma,
+                  void* workspace, cudaStream_t stream);
+// importance.cu: inverse-CDF sampling from a density grid (mvsn_sample_importance).  The coarse samples are marched
+// from rays / t_steps / jitter (t_steps set) or read from z_in / ndc_in; cams: sc's cameras are valid (needed by the
+// march and by ndc_out); sc.D / Hp / Wp are the grid's dims.
+struct ImportanceIO {
+    const float* rays; const float* t_steps; const float* jitter;
+    const float* z_in; const float* ndc_in;
+    const float* sigma; const float* u;
+    int N, S, K, cams;
+    float* z_out; float* pts_out; float* ndc_out;
+};
+constexpr int MAX_IMPORTANCE_SAMPLES = 1024;             // S + K
+int launch_importance(const SceneDev& sc, const RayGenDev& rg, const ImportanceIO& io, cudaStream_t stream);
 // fp16 [D,Hp,Wp,8] image of a planar [8,D,Hp,Wp] or channels-last volume, fp32 or fp16, rounded with __float2half_rn
 int launch_volume_to_half(const void* src, bool src_half, bool src_planar, long long nvox, void* dst, cudaStream_t stream);
 size_t mlp_wg_packed_bytes(bool split);

@@ -150,8 +150,8 @@ __device__ __forceinline__ void epilogue128(float (&acc)[8][8], const float* __r
 // Front end of row `row` (threads 0..127): sample s_idx of ray `ray`, as the caller maps rows to samples.  Fills the
 // row of sm.pe, the FEAT_LD feature row at the start of sm.h, sm.dir and sm.z; an invalid row gets zeros (and
 // cos(0) = 1 in its positional encoding).  With io.input_feat set, the 20 feature channels also go to HBM.
-// `jitter`: stratified depths for the FAST march (see sample_point).
-template <bool FAST, class Rec>
+// `jitter`: stratified depths for the FAST march (see sample_point).  VT: the volume storage (see sample_volume).
+template <bool FAST, class Rec, typename VT = float>
 __device__ __forceinline__ void tile_front_end(const SceneDev& sc, const Cams& cams, const RenderIO& io, const TileSmem& sm,
                                                int row, int ray, int s_idx, bool valid, const Rec& rec,
                                                const float* jitter = nullptr) {
@@ -163,7 +163,7 @@ __device__ __forceinline__ void tile_front_end(const SceneDev& sc, const Cams& c
         float px, py, pz, dx, dy, dz;
         sample_point<FAST, true>(sc, cams, io, ray, s_idx, si, px, py, pz, dx, dy, dz, pe[0], pe[1], pe[2], zv, jitter);
         view_dir(cams, dx, dy, dz, dir);
-        sample_volume(sc, pe[0], pe[1], pe[2], feat);
+        sample_volume<VT>(sc, pe[0], pe[1], pe[2], feat);
 #pragma unroll
         for (int v = 0; v < 3; ++v) sample_color(sc, cams, v, px, py, pz, feat + 8 + 4 * v);
         if (io.input_feat) {

@@ -39,6 +39,7 @@ EXPORTS = [
     "mvsn_occupancy_bytes", "mvsn_build_occupancy_workspace_bytes", "mvsn_build_occupancy",
     "mvsn_render_rays_occ_workspace_bytes", "mvsn_render_rays_occ",
     "mvsn_render_samples_stop", "mvsn_render_backward_stop_workspace_bytes", "mvsn_render_backward_stop",
+    "mvsn_build_density_workspace_bytes", "mvsn_build_density", "mvsn_sample_importance",
 ]
 VOLUME_F16 = 0x100       # OR-ed into RenderScene.mlp_mode (TC modes): volume_dhwc is an fp16 [D,Hp,Wp,8] image
 MAX_PEERS, PEER_HANDLE_BYTES = 16, 64
@@ -69,6 +70,10 @@ class RayParams(C.Structure):
 
 class OccupancyGrid(C.Structure):
     _fields_ = [("bits", C.c_void_p), ("D", C.c_int), ("Hp", C.c_int), ("Wp", C.c_int)]
+
+
+class DensityGrid(C.Structure):
+    _fields_ = [("sigma", C.c_void_p), ("D", C.c_int), ("Hp", C.c_int), ("Wp", C.c_int)]
 
 
 _lib = None
@@ -104,6 +109,11 @@ def load() -> C.CDLL:
         getattr(lib, name).restype = C.c_size_t
         getattr(lib, name).argtypes = [ip, ip, ip]
     lib.mvsn_build_occupancy.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), ip, vp, vp, C.c_size_t, vp]
+    lib.mvsn_build_density_workspace_bytes.restype = C.c_size_t
+    lib.mvsn_build_density_workspace_bytes.argtypes = [ip, ip, ip]
+    lib.mvsn_build_density.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), vp, vp, C.c_size_t, vp]
+    lib.mvsn_sample_importance.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), C.POINTER(DensityGrid), vp, vp,
+                                           vp, vp, vp, vp, ip, ip, ip, vp, vp, vp, vp]
     lib.mvsn_render_rays_occ_workspace_bytes.restype = C.c_size_t
     lib.mvsn_render_rays_occ_workspace_bytes.argtypes = [ip, ip]
     lib.mvsn_render_rays_occ.argtypes = [C.POINTER(RenderScene), C.POINTER(RayParams), vp, vp, ip, ip, fp,
@@ -166,7 +176,8 @@ def load() -> C.CDLL:
                  "mvsn_render_backward_rays_stop", "mvsn_adam_step",
                  "mvsn_adam_step_volume", "mvsn_featurenet_forward_bn", "mvsn_costreg_forward_bn",
                  "mvsn_volume_to_half", "mvsn_costreg_forward_f16", "mvsn_build_occupancy", "mvsn_render_rays_occ",
-                 "mvsn_render_samples_stop", "mvsn_render_backward_stop"):
+                 "mvsn_render_samples_stop", "mvsn_render_backward_stop", "mvsn_build_density",
+                 "mvsn_sample_importance"):
         getattr(lib, name).restype = ip
     _lib = lib
     return lib

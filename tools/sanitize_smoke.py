@@ -51,6 +51,19 @@ with torch.no_grad():
                 for grid in (occ, empty, full):
                     backend.render_rays(many, vol, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=128,
                                         mlp_mode=mode, t_stop=0.5, occupancy=grid, white_bkgd=True)
+                # importance sampling: the density grid (fp32 tile over the node samples, fp32 and fp16 volumes), the
+                # sampler marching the 1994 rays (S + K = 88, random draws) into the samples entry, and the sampler on
+                # given samples (ray_marcher_fine, S + K = 1024: the largest sort)
+                den = backend.build_density(vol, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad))
+                backend.build_density(vol.half(), d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad))
+                backend.render_rays(many, vol, d.imgs_raw, d.pose_source, fn, sc.near_far, float(sc.pad), N_samples=64,
+                                    mlp_mode=mode, t_stop=0.5, density=den, N_importance=24,
+                                    importance_u=torch.rand(many.shape[0], 24, device=dev))
+                xyz_i, _, _, z_i = backend.ray_marcher(many[:300], N_samples=1000)
+                ndc_i = backend.get_ndc_coordinate(d.pose_source["w2cs"][0], d.pose_source["intrinsics"][0], xyz_i,
+                                                   torch.tensor([sc.W - 1.0, sc.H - 1.0], device=dev),
+                                                   near=sc.near_far[0], far=sc.near_far[1], pad=sc.pad)
+                backend.ray_marcher_fine(many[:300], den, z_i, ndc_i, N_importance=24)
                 # fp16 volume (MVSN_VOLUME_F16): channels-last in place, then planar through mvsn_volume_to_half; both
                 # entries, the sink and the STOP instantiations
                 for vh in (vol.half(), vol.contiguous().half()):
