@@ -281,6 +281,13 @@ int mvsn_make_rays(const float* directions, const float* c2w, float near, float 
  *   grad_mlp[22]: OVERWRITTEN with d loss / d tensor, nn.Linear layouts;
  *   grad_volume_dhwc: [D,Hp,Wp,8] channels-last, ACCUMULATED (atomics); NULL = volume frozen;
  *   workspace: mvsn_render_backward_workspace_bytes(N, S) bytes, 16-byte aligned.
+ * Every mvsn_render_backward* entry returns its argument errors before any CUDA call, checked in this order: a
+ *   grad_mode the entry does not take (MVSN_EUNSUPPORTED); the scene; NULL pointers (MVSN_ENULL); with t_stop (the
+ *   _stop entries), t_stop negative, NaN or > 1 (MVSN_EBADSHAPE), then g->weights / g->alpha / g->input_feat set
+ *   (MVSN_EUNSUPPORTED: per-sample cotangents of dead samples are not defined); a misaligned rays, grad_volume_dhwc,
+ *   live_samples or tiles_done (MVSN_EALIGN); N < 0 or N_samples < 1 (MVSN_EBADSHAPE); N_samples > 128
+ *   (MVSN_EUNSUPPORTED); scene->mlp_packed not the MVSN_MLP_FP32 image (MVSN_EUNSUPPORTED).  N == 0 then returns
+ *   MVSN_OK.
  * mvsn_adam_step / mvsn_adam_step_volume: torch.optim.Adam arithmetic (betas, eps, bias correction by `step` >= 1,
  *   no weight decay / amsgrad).  The volume variant reads the channels-last gradient, zeroes it for the next step,
  *   and updates a parameter (and moments) stored channels-last (planar = 0) or planar [8][nvox] (planar = 1).
@@ -342,8 +349,7 @@ int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const flo
  * rgb_out / depth_out / the loss are then this mode's forward); deterministic != 0 sums the volume gradient and the loss as
  * mvsn_render_backward_deterministic does.  g, grad_mlp and grad_volume_dhwc as mvsn_render_backward; rgb_out /
  * depth_out receive the forward of the marched samples (with jitter = NULL: rgb bit-identical to mvsn_render_rays with
- * the MVSN_MLP_FP32 image).  N_samples <= 128.  Argument errors are returned before any CUDA call: an unknown grad_mode
- * (MVSN_EUNSUPPORTED) first, then NULL pointers, a misaligned rays, then N_samples > 128 (MVSN_EUNSUPPORTED).
+ * the MVSN_MLP_FP32 image).  N_samples <= 128.  Argument errors: see the head of this section.
  * Workspace: mvsn_render_backward_rays_workspace_bytes(N, S, D, Hp, Wp, grad_mode, deterministic) bytes, 16-byte
  * aligned; the volume dims matter only with `deterministic` (D = Hp = Wp = 0: a frozen volume).  0 for an unknown
  * grad_mode or shape. */
@@ -363,11 +369,9 @@ int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const
  * summation order only.  deterministic != 0: every output is a deterministic function of the inputs.
  * live_samples [N] int32 (device, 4-byte aligned, may be NULL): each ray's L.  tiles_done (device, 8-byte aligned, may
  * be NULL): unsigned long long[3] += the 128-row tiles back-propagated immediately, deferred, and packed from deferred
- * rays.  Everything else as mvsn_render_backward_rays.  Argument errors are returned before any CUDA call: an unknown
- * grad_mode, NULL pointers, t_stop negative, NaN or > 1 (MVSN_EBADSHAPE), g->weights / g->alpha / g->input_feat set
- * (MVSN_EUNSUPPORTED: per-sample cotangents of dead samples are not defined), a misaligned rays, live_samples or
- * tiles_done, then N_samples > 128 (MVSN_EUNSUPPORTED).  Workspace: mvsn_render_backward_rays_stop_workspace_bytes(N,
- * S, D, Hp, Wp, grad_mode, deterministic) bytes, 16-byte aligned (a little more than mvsn_render_backward_rays'). */
+ * rays.  Everything else as mvsn_render_backward_rays; argument errors: see the head of this section.  Workspace:
+ * mvsn_render_backward_rays_stop_workspace_bytes(N, S, D, Hp, Wp, grad_mode, deterministic) bytes, 16-byte aligned (a
+ * little more than mvsn_render_backward_rays'). */
 size_t mvsn_render_backward_rays_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode,
                                                       int deterministic);
 int mvsn_render_backward_rays_stop(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
@@ -389,10 +393,8 @@ int mvsn_render_backward_rays_stop(const mvsn_render_scene* scene, const float* 
  * mvsn_render_backward_deterministic sums them.  Inputs, g, grad_mlp and grad_volume_dhwc as mvsn_render_backward;
  * N_samples <= 128.  live_samples [N] int32 (device, 4-byte aligned, may be NULL): each ray's L.  tiles_done (device,
  * 8-byte aligned, may be NULL): unsigned long long[3] += the 128-row tiles back-propagated immediately, deferred, and
- * packed from deferred rays.  Argument errors are returned before any CUDA call: a grad_mode other than MVSN_MLP_FP32
- * or MVSN_MLP_TC_HALF (MVSN_EUNSUPPORTED), NULL pointers, t_stop negative, NaN or > 1 (MVSN_EBADSHAPE), g->weights /
- * g->alpha / g->input_feat set (MVSN_EUNSUPPORTED: per-sample cotangents of dead samples are not defined), a misaligned
- * grad_volume_dhwc, live_samples or tiles_done, then N_samples > 128 (MVSN_EUNSUPPORTED).  Workspace:
+ * packed from deferred rays.  grad_mode MVSN_MLP_FP32 or MVSN_MLP_TC_HALF; argument errors: see the head of this
+ * section.  Workspace:
  * mvsn_render_backward_stop_workspace_bytes(N, S, D, Hp, Wp, grad_mode, deterministic) bytes, 16-byte aligned; the
  * volume dims matter only with `deterministic` (D = Hp = Wp = 0: a frozen volume).  0 for an unknown grad_mode or
  * shape. */

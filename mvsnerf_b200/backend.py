@@ -652,21 +652,15 @@ class _RenderSamplesFn(torch.autograd.Function):
                                    "and take no cotangent")
             if S > 128 or BACKWARD_IMPL != "kernel":
                 raise RuntimeError(f"rendering with t_stop: the backward kernel takes N_samples <= 128 (got {S})")
-            need_vol = ctx.needs_input_grad[4]
-            g_params, dvol, _, _ = render_backward(
-                {"w2cs": w2cs, "intrinsics": intrinsics}, pts, ndc, z, rays_dir, ctx.volume_feature, imgs, ctx.network_fn,
-                ctx.white_bkgd, grads={"rgb": g_rgb, "depth": g_depth}, want_volume_grad=need_vol,
-                grad_mode=ctx.grad_mode, t_stop=ctx.t_stop)
-            g_vol = dvol.permute(3, 0, 1, 2).unsqueeze(0) if need_vol else None
-            g_params = [g if need else None for g, need in zip(g_params, ctx.needs_input_grad[13:])]
-            return (None, None, None, None, g_vol, None, None, None, None, None, None, None, None, *g_params)
         if S <= 128 and BACKWARD_IMPL == "kernel":
             # the hand-written backward kernel (csrc/render_bwd.cu): recompute + dgrad/wgrad + volume scatter
             need_vol = ctx.needs_input_grad[4]
-            grads = {"rgb": g_rgb, "depth": g_depth, "weights": g_weights, "alpha": g_alpha, "input_feat": g_feat}
+            grads = {"rgb": g_rgb, "depth": g_depth}
+            if ctx.t_stop is None:
+                grads.update(weights=g_weights, alpha=g_alpha, input_feat=g_feat)
             g_params, dvol, _, _ = render_backward(
                 {"w2cs": w2cs, "intrinsics": intrinsics}, pts, ndc, z, rays_dir, ctx.volume_feature, imgs, ctx.network_fn,
-                ctx.white_bkgd, grads=grads, want_volume_grad=need_vol, grad_mode=ctx.grad_mode)
+                ctx.white_bkgd, grads=grads, want_volume_grad=need_vol, grad_mode=ctx.grad_mode, t_stop=ctx.t_stop)
             g_vol = dvol.permute(3, 0, 1, 2).unsqueeze(0) if need_vol else None
             g_params = [g if need else None for g, need in zip(g_params, ctx.needs_input_grad[13:])]
             return (None, None, None, None, g_vol, None, None, None, None, None, None, None, None, *g_params)
@@ -706,24 +700,60 @@ def _check_grad_mode(grad_mode, rays=False):
                            "(wgmma, fp16 operands with per-tile power-of-two scales, fp32 accumulation)")
 
 
-def _backward_workspace(dev, N, S, grad_mode=_lib.MLP_FP32, det_volume=None):
-    """The shared backward workspace, grown to this call's need.  det_volume = (D, Hp, Wp) of the volume gradient, or
-    (0, 0, 0) for a frozen volume, sizes it for mvsn_render_backward_deterministic instead."""
+def _backward(who, rays, inputs, dev, N, S, pose_ref, volume_feature, imgs, network_fn, white_bkgd, grads, target_rgb,
+              n_total, want_volume_grad, grad_volume, grad_mlp, want_forward, loss_out, grad_mode, t_stop, live_samples,
+              tiles_done):
+    """One launch of a backward C entry over N rays x S samples on `dev`: render_backward (`rays` False) or
+    render_backward_rays (`who`).  Every argument is checked before `inputs()` prepares the entry's own: it returns the
+    C arguments between the weights and N, and the objects they point into."""
+    _check_grad_mode(grad_mode, rays)
+    if t_stop is not None:
+        t_stop = float(t_stop)
+        if not 0.0 <= t_stop <= 1.0:
+            raise RuntimeError(f"{who}: t_stop={t_stop} must be in [0, 1]")
+        if grads is not None and any(grads.get(k) is not None for k in ("weights", "alpha", "input_feat")):
+            raise RuntimeError(f"{who}: t_stop takes no per-sample cotangents (weights / alpha / input_feat):"
+                               " dead samples have none")
+        _check_counter(live_samples, who, "live_samples", torch.int32, N, dev)
+        _check_counter(tiles_done, who, "tiles_done", torch.int64, 3, dev)
+    elif live_samples is not None or tiles_done is not None:
+        raise RuntimeError(f"{who}: live_samples / tiles_done need t_stop")
     lib = _lib.load()
-    if det_volume is not None:
-        need = lib.mvsn_render_backward_deterministic_workspace_bytes(int(N), int(S), *[int(v) for v in det_volume],
-                                                                     int(grad_mode))
-    elif grad_mode == _lib.MLP_TC_HALF:
-        need = lib.mvsn_render_backward_tc_workspace_bytes(int(N), int(S))
+    args, held_inputs = inputs()
+    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, _lib.MLP_FP32)
+    params = [_lib.dev_f32(p.detach(), "MLP parameter") for p in network_fn.ordered_params()]
+    if grad_mlp is None:
+        grad_mlp = [torch.empty_like(p) for p in params]
+    if want_volume_grad and grad_volume is None:
+        grad_volume = torch.zeros(sc.D, sc.Hp, sc.Wp, 8, dtype=torch.float32, device=dev)
+    g, held, rgb, depth = _render_grads(N, S, dev, grads, target_rgb, n_total, want_forward, loss_out)
+    det = torch.are_deterministic_algorithms_enabled()
+    dims = (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0)
+    # mvsn_render_backward_rays[_stop] and mvsn_render_backward_stop take (grad_mode, deterministic[, t_stop]); the
+    # other samples entries are named by their summation order, and by their grad mode unless deterministic
+    if rays or t_stop is not None:
+        name = "mvsn_render_backward" + ("_rays" if rays else "") + ("_stop" if t_stop is not None else "")
+        modes = (int(grad_mode), int(det)) + (() if t_stop is None else (t_stop,))
+        need = getattr(lib, name + "_workspace_bytes")(N, S, *dims, int(grad_mode), int(det))
+    elif det:
+        name, modes = "mvsn_render_backward_deterministic", (int(grad_mode),)
+        need = lib.mvsn_render_backward_deterministic_workspace_bytes(N, S, *dims, int(grad_mode))
     else:
-        need = lib.mvsn_render_backward_workspace_bytes(int(N), int(S))
+        name = "mvsn_render_backward_tc" if grad_mode == _lib.MLP_TC_HALF else "mvsn_render_backward"
+        modes, need = (), getattr(lib, name + "_workspace_bytes")(N, S)
     if need == 0:
-        raise RuntimeError(f"render backward: unsupported shape N={N}, N_samples={S} (N_samples <= 128)")
+        raise RuntimeError(f"{who}: unsupported shape N={N}, N_samples={S} (N_samples <= 128)")
     ws = _bwd_workspace.get(dev)
     if ws is None or ws.numel() < need:
         ws = torch.empty(need, dtype=torch.uint8, device=dev)
         _bwd_workspace[dev] = ws
-    return ws, need
+    counters = () if t_stop is None else (_lib.ptr(live_samples), _lib.ptr(tiles_done))
+    with torch.cuda.device(dev):
+        _lib.check(getattr(lib, name)(C.byref(sc), _lib.ptr_array(params), *args, N, S, *modes, C.byref(g),
+                                      _lib.ptr_array(grad_mlp), _lib.ptr(grad_volume) if want_volume_grad else None,
+                                      *counters, _lib.ptr(ws), need, _lib.stream_ptr()), name)
+    del keep, held, held_inputs
+    return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
 
 
 def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_feature, imgs, network_fn, white_bkgd=False,
@@ -749,68 +779,17 @@ def render_backward(pose_ref, rays_pts, rays_ndc, z_vals, rays_dir, volume_featu
     'alpha', 'input_feat') are rejected with it.  `live_samples`: an optional CUDA int32 tensor [N] that receives each
     ray's number of kept samples; `tiles_done`: an optional CUDA int64 tensor [3] the counts of tiles back-propagated
     immediately, deferred and packed are added to."""
-    _check_grad_mode(grad_mode)
     N, S = rays_pts.shape[:2]
-    dev = rays_pts.device
-    if t_stop is not None:
-        t_stop = float(t_stop)
-        if not 0.0 <= t_stop <= 1.0:
-            raise RuntimeError(f"render_backward: t_stop={t_stop} must be in [0, 1]")
-        if grads is not None and any(grads.get(k) is not None for k in ("weights", "alpha", "input_feat")):
-            raise RuntimeError("render_backward: t_stop takes no per-sample cotangents (weights / alpha / input_feat):"
-                               " dead samples have none")
-        _check_counter(live_samples, "render_backward", "live_samples", torch.int32, N, dev)
-        _check_counter(tiles_done, "render_backward", "tiles_done", torch.int64, 3, dev)
-    elif live_samples is not None or tiles_done is not None:
-        raise RuntimeError("render_backward: live_samples / tiles_done need t_stop")
-    lib = _lib.load()
-    pts = _lib.dev_f32(rays_pts.detach(), "rays_pts")
-    ndc = _lib.dev_f32(rays_ndc.detach(), "rays_ndc")
-    z = _lib.dev_f32((z_vals.expand(N, S) if z_vals.shape != (N, S) else z_vals).detach(), "depth_candidates")
-    dirs = _lib.dev_f32(rays_dir.detach(), "rays_dir")
-    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, _lib.MLP_FP32)
-    params = [_lib.dev_f32(p.detach(), "MLP parameter") for p in network_fn.ordered_params()]
-    if grad_mlp is None:
-        grad_mlp = [torch.empty_like(p) for p in params]
-    if want_volume_grad and grad_volume is None:
-        grad_volume = torch.zeros(sc.D, sc.Hp, sc.Wp, 8, dtype=torch.float32, device=dev)
-    g, held, rgb, depth = _render_grads(N, S, dev, grads, target_rgb, n_total, want_forward, loss_out)
-    vol_arg = _lib.ptr(grad_volume) if want_volume_grad else None
-    if t_stop is not None:
-        det = torch.are_deterministic_algorithms_enabled()
-        dims = (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0)
-        need = lib.mvsn_render_backward_stop_workspace_bytes(int(N), int(S), *dims, int(grad_mode), int(det))
-        if need == 0:
-            raise RuntimeError(f"render backward: unsupported shape N={N}, N_samples={S} (N_samples <= 128)")
-        ws = _bwd_workspace.get(dev)
-        if ws is None or ws.numel() < need:
-            ws = torch.empty(need, dtype=torch.uint8, device=dev)
-            _bwd_workspace[dev] = ws
-        with torch.cuda.device(dev):
-            _lib.check(lib.mvsn_render_backward_stop(
-                C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z), _lib.ptr(dirs), N, S,
-                int(grad_mode), int(det), t_stop, C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(live_samples),
-                _lib.ptr(tiles_done), _lib.ptr(ws), need, _lib.stream_ptr()), "mvsn_render_backward_stop")
-        del keep, held
-        return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
-    if torch.are_deterministic_algorithms_enabled():
-        ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode, (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0))
-        with torch.cuda.device(dev):
-            _lib.check(lib.mvsn_render_backward_deterministic(
-                C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z), _lib.ptr(dirs), N, S,
-                int(grad_mode), C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(ws), ws_bytes,
-                _lib.stream_ptr()), "mvsn_render_backward_deterministic")
-        del keep, held
-        return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
-    ws, ws_bytes = _backward_workspace(dev, N, S, grad_mode)
-    entry, name = ((lib.mvsn_render_backward_tc, "mvsn_render_backward_tc") if grad_mode == _lib.MLP_TC_HALF
-                   else (lib.mvsn_render_backward, "mvsn_render_backward"))
-    with torch.cuda.device(dev):
-        _lib.check(entry(C.byref(sc), _lib.ptr_array(params), _lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z),
-                         _lib.ptr(dirs), N, S, C.byref(g), _lib.ptr_array(grad_mlp), vol_arg, _lib.ptr(ws), ws_bytes,
-                         _lib.stream_ptr()), name)
-    del keep, held
-    return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
+
+    def inputs():
+        pts = _lib.dev_f32(rays_pts.detach(), "rays_pts")
+        ndc = _lib.dev_f32(rays_ndc.detach(), "rays_ndc")
+        z = _lib.dev_f32((z_vals.expand(N, S) if z_vals.shape != (N, S) else z_vals).detach(), "depth_candidates")
+        dirs = _lib.dev_f32(rays_dir.detach(), "rays_dir")
+        return (_lib.ptr(pts), _lib.ptr(ndc), _lib.ptr(z), _lib.ptr(dirs)), (pts, ndc, z, dirs)
+    return _backward("render_backward", False, inputs, rays_pts.device, N, S, pose_ref, volume_feature, imgs, network_fn,
+                     white_bkgd, grads, target_rgb, n_total, want_volume_grad, grad_volume, grad_mlp, want_forward,
+                     loss_out, grad_mode, t_stop, live_samples, tiles_done)
 
 
 def _render_grads(N, S, dev, grads, target_rgb, n_total, want_forward, loss_out):
@@ -882,61 +861,18 @@ def render_backward_rays(rays, volume_feature, imgs, pose_ref, network_fn, near_
     grad_mode=GRAD_TC_FULL: MLP_TC_HALF's backward, and the forward recompute's MLP on tensor cores too (fp16 operands,
     a power-of-two scale per sample row, fp32 accumulation; see MVSN_GRAD_TC_FULL in include/mvsnerf_b200.h).  rgb,
     depth and the loss are then that recompute's, within the 5e-3 tier of MLP_FP32."""
-    _check_grad_mode(grad_mode, rays=True)
-    if t_stop is not None:
-        t_stop = float(t_stop)
-        if not 0.0 <= t_stop <= 1.0:
-            raise RuntimeError(f"render_backward_rays: t_stop={t_stop} must be in [0, 1]")
-        if grads is not None and any(grads.get(k) is not None for k in ("weights", "alpha", "input_feat")):
-            raise RuntimeError("render_backward_rays: t_stop takes no per-sample cotangents (weights / alpha / input_feat):"
-                               " dead samples have none")
-        for t, name, dtype, n in ((live_samples, "live_samples", torch.int32, rays.shape[0]), (tiles_done, "tiles_done", torch.int64, 3)):
-            if t is not None and (not t.is_cuda or t.device != rays.device or t.dtype != dtype or t.numel() < n
-                                  or not t.is_contiguous()):
-                raise RuntimeError(f"render_backward_rays: {name} must be a contiguous CUDA {dtype} tensor of >= {n} "
-                                   f"elements on the rays' device ({rays.device})")
-    elif live_samples is not None or tiles_done is not None:
-        raise RuntimeError("render_backward_rays: live_samples / tiles_done need t_stop")
-    lib = _lib.load()
-    rays = _lib.dev_f32(rays.detach(), "rays")
     N, S = rays.shape[0], int(N_samples)
-    dev = rays.device
-    if jitter is not None:
-        jitter = _lib.dev_f32(jitter.detach(), "jitter")
-        if tuple(jitter.shape) != (N, S):
-            raise RuntimeError(f"render_backward_rays: jitter must be [{N}, {S}], got {tuple(jitter.shape)}")
-    sc, keep = _make_scene(pose_ref, volume_feature, imgs, network_fn, white_bkgd, _lib.MLP_FP32)
-    rp = _lib.RayParams(float(near_far[0]), float(near_far[1]), float(pad), int(bool(lindisp)))
-    params = [_lib.dev_f32(p.detach(), "MLP parameter") for p in network_fn.ordered_params()]
-    if grad_mlp is None:
-        grad_mlp = [torch.empty_like(p) for p in params]
-    if want_volume_grad and grad_volume is None:
-        grad_volume = torch.zeros(sc.D, sc.Hp, sc.Wp, 8, dtype=torch.float32, device=dev)
-    g, held, rgb, depth = _render_grads(N, S, dev, grads, target_rgb, n_total, want_forward, loss_out)
-    det = torch.are_deterministic_algorithms_enabled()
-    dims = (sc.D, sc.Hp, sc.Wp) if want_volume_grad else (0, 0, 0)
-    ws_bytes = (lib.mvsn_render_backward_rays_workspace_bytes if t_stop is None
-                else lib.mvsn_render_backward_rays_stop_workspace_bytes)
-    need = ws_bytes(N, S, *dims, int(grad_mode), int(det))
-    if need == 0:
-        raise RuntimeError(f"render_backward_rays: unsupported shape N={N}, N_samples={S} (N_samples <= 128)")
-    ws = _bwd_workspace.get(dev)
-    if ws is None or ws.numel() < need:
-        ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        _bwd_workspace[dev] = ws
-    head = (C.byref(sc), _lib.ptr_array(params), C.byref(rp), _lib.ptr(rays), _lib.ptr(_tsteps_of(S, dev)),
-            _lib.ptr(jitter), N, S, int(grad_mode), int(det))
-    tail = (C.byref(g), _lib.ptr_array(grad_mlp), _lib.ptr(grad_volume) if want_volume_grad else None)
-    with torch.cuda.device(dev):
-        if t_stop is None:
-            _lib.check(lib.mvsn_render_backward_rays(*head, *tail, _lib.ptr(ws), need, _lib.stream_ptr()),
-                       "mvsn_render_backward_rays")
-        else:
-            _lib.check(lib.mvsn_render_backward_rays_stop(*head, t_stop, *tail, _lib.ptr(live_samples),
-                                                          _lib.ptr(tiles_done), _lib.ptr(ws), need, _lib.stream_ptr()),
-                       "mvsn_render_backward_rays_stop")
-    del keep, held
-    return grad_mlp, (grad_volume if want_volume_grad else None), rgb, depth
+
+    def inputs():
+        r = _lib.dev_f32(rays.detach(), "rays")
+        j = None if jitter is None else _lib.dev_f32(jitter.detach(), "jitter")
+        if j is not None and tuple(j.shape) != (N, S):
+            raise RuntimeError(f"render_backward_rays: jitter must be [{N}, {S}], got {tuple(j.shape)}")
+        rp = _lib.RayParams(float(near_far[0]), float(near_far[1]), float(pad), int(bool(lindisp)))
+        return (C.byref(rp), _lib.ptr(r), _lib.ptr(_tsteps_of(S, r.device)), _lib.ptr(j)), (rp, r, j)
+    return _backward("render_backward_rays", True, inputs, rays.device, N, S, pose_ref, volume_feature, imgs, network_fn,
+                     white_bkgd, grads, target_rgb, n_total, want_volume_grad, grad_volume, grad_mlp, want_forward,
+                     loss_out, grad_mode, t_stop, live_samples, tiles_done)
 
 
 class FineTuner:

@@ -511,143 +511,38 @@ int mvsn_make_rays(const float* directions, const float* c2w, float near, float 
 }
 
 // ---- fine-tuning step ------------------------------------------------------------------------------------
-size_t mvsn_render_backward_workspace_bytes(int N, int S) { return render_backward_workspace_bytes(N, S); }
-size_t mvsn_render_backward_tc_workspace_bytes(int N, int S) { return render_backward_tc_workspace_bytes(N, S); }
-size_t mvsn_render_backward_deterministic_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode) {
-    if (grad_mode != MVSN_MLP_FP32 && grad_mode != MVSN_MLP_TC_HALF) return 0;
-    return render_backward_det_workspace_bytes(N, S, D, Hp, Wp, grad_mode);
+// The grad modes of the backward entries: MVSN_GRAD_TC_FULL marches its samples in the kernel, so only the rays
+// entries take it.
+static bool backward_grad_mode(int grad_mode, bool rays) {
+    return grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF || (rays && grad_mode == MVSN_GRAD_TC_FULL);
 }
 
-static int render_backward_entry(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
-                                 const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
-                                 const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc,
-                                 void* workspace, size_t workspace_bytes, void* stream, bool tc, bool det = false) {
+static size_t backward_bytes(bool rays, int N, int S, int D, int Hp, int Wp, int grad_mode, bool det, bool stop) {
+    return backward_grad_mode(grad_mode, rays) ? backward_layout(N, S, D, Hp, Wp, grad_mode, det, stop).total : 0;
+}
+
+// The inputs of a backward entry: the samples (pts, ndc, z, dirs) or, rp set, the rays marched in the kernel.
+struct BwdInputs {
+    const float *pts, *ndc, *z, *dirs;
+    const mvsn_ray_params* rp; const float *rays, *t_steps, *jitter;
+};
+
+// Every backward entry, with its checks in the order include/mvsnerf_b200.h states for the fine-tuning entries.
+static int backward_entry(const char* what, bool rays, const mvsn_render_scene* scene, const float* const* mlp_w,
+                          const BwdInputs& in, int N, int S, int grad_mode, bool det, const BwdStop* stop,
+                          const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+    MVSN_REQUIRE(backward_grad_mode(grad_mode, rays), MVSN_EUNSUPPORTED, "%s: grad_mode %d (%s)", what, grad_mode,
+                 rays ? "MVSN_MLP_FP32, MVSN_MLP_TC_HALF or MVSN_GRAD_TC_FULL" : "MVSN_MLP_FP32 or MVSN_MLP_TC_HALF");
     SceneDev sc;
     int rc = make_scene(scene, sc);
     if (rc) return rc;
-    MVSN_REQUIRE(scene->mlp_mode == MVSN_MLP_FP32, MVSN_EUNSUPPORTED,
-                 "mvsn_render_backward: scene->mlp_packed must be the MVSN_MLP_FP32 image (mode %d given)", scene->mlp_mode);
-    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "mvsn_render_backward: N=%d S=%d", N, S);
-    MVSN_REQUIRE(g && mlp_w && grad_mlp, MVSN_ENULL, "mvsn_render_backward: NULL argument");
-    MVSN_REQUIRE(g->rgb || g->target_rgb, MVSN_ENULL, "mvsn_render_backward: neither g->rgb nor g->target_rgb given");
-    for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i)
-        MVSN_REQUIRE(mlp_w[i] && grad_mlp[i], MVSN_ENULL, "mvsn_render_backward: tensor %d is NULL", i);
-    MVSN_REQUIRE(!grad_volume_dhwc || aligned16(grad_volume_dhwc), MVSN_EALIGN, "grad_volume_dhwc must be 16-byte aligned");
-    if (N == 0) return MVSN_OK;
-    MVSN_REQUIRE(rays_pts && rays_ndc && z_vals && rays_dir, MVSN_ENULL, "mvsn_render_backward: NULL required pointer");
-    RenderIO io{};
-    io.pts = rays_pts; io.ndc = rays_ndc; io.z = z_vals; io.dirs = rays_dir;
-    io.N = N; io.S = S;
-    return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
-                                  g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
-                                  grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
-                                  (cudaStream_t)stream, tc ? MVSN_MLP_TC_HALF : MVSN_MLP_FP32, det);
-}
-
-int mvsn_render_backward(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
-                         const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
-                         const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
-                         size_t workspace_bytes, void* stream) {
-    MVSN_RANGE("mvsn_render_backward");
-    return render_backward_entry(scene, mlp_w, rays_pts, rays_ndc, z_vals, rays_dir, N, S, g, grad_mlp, grad_volume_dhwc,
-                                 workspace, workspace_bytes, stream, false);
-}
-
-int mvsn_render_backward_tc(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
-                            const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
-                            const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
-                            size_t workspace_bytes, void* stream) {
-    MVSN_RANGE("mvsn_render_backward_tc");
-    return render_backward_entry(scene, mlp_w, rays_pts, rays_ndc, z_vals, rays_dir, N, S, g, grad_mlp, grad_volume_dhwc,
-                                 workspace, workspace_bytes, stream, true);
-}
-
-int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
-                                       const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
-                                       int grad_mode, const mvsn_render_grads* g, float* const* grad_mlp,
-                                       float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream) {
-    MVSN_RANGE("mvsn_render_backward_deterministic");
-    MVSN_REQUIRE(grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF, MVSN_EUNSUPPORTED,
-                 "mvsn_render_backward_deterministic: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)", grad_mode);
-    return render_backward_entry(scene, mlp_w, rays_pts, rays_ndc, z_vals, rays_dir, N, S, g, grad_mlp, grad_volume_dhwc,
-                                 workspace, workspace_bytes, stream, grad_mode == MVSN_MLP_TC_HALF, true);
-}
-
-// the grad modes of the samples entries
-static bool samples_grad_mode(int grad_mode) { return grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF; }
-
-size_t mvsn_render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
-    if (!samples_grad_mode(grad_mode)) return 0;
-    return render_backward_stop_workspace_bytes(N, S, D, Hp, Wp, grad_mode, deterministic != 0);
-}
-
-int mvsn_render_backward_stop(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
-                              const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
-                              int grad_mode, int deterministic, float t_stop, const mvsn_render_grads* g,
-                              float* const* grad_mlp, float* grad_volume_dhwc, int* live_samples,
-                              unsigned long long* tiles_done, void* workspace, size_t workspace_bytes, void* stream) {
-    MVSN_RANGE("mvsn_render_backward_stop");
-    const char* what = "mvsn_render_backward_stop";
-    MVSN_REQUIRE(samples_grad_mode(grad_mode), MVSN_EUNSUPPORTED, "%s: grad_mode %d (MVSN_MLP_FP32 or MVSN_MLP_TC_HALF)",
-                 what, grad_mode);
-    SceneDev sc;
-    int rc = make_scene(scene, sc);
-    if (rc) return rc;
-    MVSN_REQUIRE(g && mlp_w && grad_mlp, MVSN_ENULL, "%s: NULL argument", what);
+    MVSN_REQUIRE((!rays || in.rp) && g && mlp_w && grad_mlp, MVSN_ENULL, "%s: NULL argument", what);
     MVSN_REQUIRE(g->rgb || g->target_rgb, MVSN_ENULL, "%s: neither g->rgb nor g->target_rgb given", what);
     for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i)
         MVSN_REQUIRE(mlp_w[i] && grad_mlp[i], MVSN_ENULL, "%s: tensor %d is NULL", what, i);
-    MVSN_REQUIRE(N == 0 || (rays_pts && rays_ndc && z_vals && rays_dir), MVSN_ENULL, "%s: NULL required pointer", what);
-    MVSN_REQUIRE(t_stop >= 0.f && t_stop <= 1.f, MVSN_EBADSHAPE, "%s: t_stop=%g must be in [0, 1] (not NaN)", what,
-                 (double)t_stop);
-    MVSN_REQUIRE(!g->weights && !g->alpha && !g->input_feat, MVSN_EUNSUPPORTED,
-                 "%s: g->weights / g->alpha / g->input_feat are per-sample cotangents, not defined for dead samples", what);
-    MVSN_REQUIRE(!grad_volume_dhwc || aligned16(grad_volume_dhwc), MVSN_EALIGN, "grad_volume_dhwc must be 16-byte aligned");
-    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(live_samples) % 4 == 0, MVSN_EALIGN, "%s: live_samples must be 4-byte aligned",
-                 what);
-    MVSN_REQUIRE(reinterpret_cast<uintptr_t>(tiles_done) % 8 == 0, MVSN_EALIGN, "%s: tiles_done must be 8-byte aligned", what);
-    MVSN_REQUIRE(N >= 0 && S > 0, MVSN_EBADSHAPE, "%s: N=%d S=%d", what, N, S);
-    MVSN_REQUIRE(S <= 128, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, S);
-    MVSN_REQUIRE(scene->mlp_mode == MVSN_MLP_FP32, MVSN_EUNSUPPORTED,
-                 "%s: scene->mlp_packed must be the MVSN_MLP_FP32 image (mode %d given)", what, scene->mlp_mode);
-    if (N == 0) return MVSN_OK;
-    RenderIO io{};
-    io.pts = rays_pts; io.ndc = rays_ndc; io.z = z_vals; io.dirs = rays_dir;
-    io.N = N; io.S = S;
-    const BwdStop stop{t_stop, live_samples, tiles_done};
-    return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
-                                  g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
-                                  grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
-                                  (cudaStream_t)stream, grad_mode, deterministic != 0, nullptr, &stop);
-}
-
-// the grad modes of the rays entries
-static bool rays_grad_mode(int grad_mode) {
-    return grad_mode == MVSN_MLP_FP32 || grad_mode == MVSN_MLP_TC_HALF || grad_mode == MVSN_GRAD_TC_FULL;
-}
-
-size_t mvsn_render_backward_rays_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
-    if (!rays_grad_mode(grad_mode)) return 0;
-    if (deterministic) return render_backward_det_workspace_bytes(N, S, D, Hp, Wp, grad_mode);
-    return render_backward_mode_workspace_bytes(N, S, grad_mode);
-}
-
-// mvsn_render_backward_rays and, with `stop`, mvsn_render_backward_rays_stop (`what`: the entry's name for messages)
-static int backward_rays_entry(const char* what, const mvsn_render_scene* scene, const float* const* mlp_w,
-                               const mvsn_ray_params* rp, const float* rays, const float* t_steps, const float* jitter,
-                               int N, int S, int grad_mode, int deterministic, const mvsn_render_grads* g,
-                               float* const* grad_mlp, float* grad_volume_dhwc, void* workspace, size_t workspace_bytes,
-                               void* stream, const BwdStop* stop) {
-    MVSN_REQUIRE(rays_grad_mode(grad_mode), MVSN_EUNSUPPORTED,
-                 "%s: grad_mode %d (MVSN_MLP_FP32, MVSN_MLP_TC_HALF or MVSN_GRAD_TC_FULL)", what, grad_mode);
-    SceneDev sc;
-    int rc = make_scene(scene, sc);
-    if (rc) return rc;
-    MVSN_REQUIRE(rp && g && mlp_w && grad_mlp, MVSN_ENULL, "%s: NULL argument", what);
-    MVSN_REQUIRE(g->rgb || g->target_rgb, MVSN_ENULL, "%s: neither g->rgb nor g->target_rgb given", what);
-    for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i)
-        MVSN_REQUIRE(mlp_w[i] && grad_mlp[i], MVSN_ENULL, "%s: tensor %d is NULL", what, i);
-    MVSN_REQUIRE(N == 0 || (rays && t_steps), MVSN_ENULL, "%s: rays or t_steps is NULL", what);
+    if (rays) MVSN_REQUIRE(N == 0 || (in.rays && in.t_steps), MVSN_ENULL, "%s: rays or t_steps is NULL", what);
+    else MVSN_REQUIRE(N == 0 || (in.pts && in.ndc && in.z && in.dirs), MVSN_ENULL, "%s: NULL required pointer", what);
     if (stop) {
         MVSN_REQUIRE(stop->t_stop >= 0.f && stop->t_stop <= 1.f, MVSN_EBADSHAPE,
                      "%s: t_stop=%g must be in [0, 1] (not NaN)", what, (double)stop->t_stop);
@@ -655,7 +550,7 @@ static int backward_rays_entry(const char* what, const mvsn_render_scene* scene,
                      "%s: g->weights / g->alpha / g->input_feat are per-sample cotangents, not defined for dead samples",
                      what);
     }
-    MVSN_REQUIRE(aligned16(rays), MVSN_EALIGN, "%s: rays must be 16-byte aligned", what);
+    MVSN_REQUIRE(aligned16(in.rays), MVSN_EALIGN, "%s: rays must be 16-byte aligned", what);
     MVSN_REQUIRE(!grad_volume_dhwc || aligned16(grad_volume_dhwc), MVSN_EALIGN, "grad_volume_dhwc must be 16-byte aligned");
     if (stop) {
         MVSN_REQUIRE(reinterpret_cast<uintptr_t>(stop->live_samples) % 4 == 0, MVSN_EALIGN,
@@ -669,29 +564,84 @@ static int backward_rays_entry(const char* what, const mvsn_render_scene* scene,
                  "%s: scene->mlp_packed must be the MVSN_MLP_FP32 image (mode %d given)", what, scene->mlp_mode);
     if (N == 0) return MVSN_OK;
     RenderIO io{};
-    io.rays = rays; io.t_steps = t_steps;
-    io.rg = make_ray_gen(scene, rp);
+    io.pts = in.pts; io.ndc = in.ndc; io.z = in.z; io.dirs = in.dirs;
+    io.rays = in.rays; io.t_steps = in.t_steps;
+    if (rays) io.rg = make_ray_gen(scene, in.rp);
     io.N = N; io.S = S;
-    return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), mlp_w, g->rgb, g->target_rgb,
-                                  g->loss_scale, g->depth, g->weights, g->alpha, g->input_feat, grad_mlp,
-                                  grad_volume_dhwc, g->rgb_out, g->depth_out, g->loss_out, workspace, workspace_bytes,
-                                  (cudaStream_t)stream, grad_mode, deterministic != 0, jitter, stop);
+    const BwdCall call{what, g, mlp_w, grad_mlp, grad_volume_dhwc, workspace, workspace_bytes, grad_mode, det, in.jitter,
+                       stop};
+    return launch_render_backward(sc, io, static_cast<const float*>(scene->mlp_packed), call, (cudaStream_t)stream);
 }
 
+size_t mvsn_render_backward_workspace_bytes(int N, int S) {
+    return backward_bytes(false, N, S, 0, 0, 0, MVSN_MLP_FP32, false, false);
+}
+int mvsn_render_backward(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                         const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                         const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward");
+    return backward_entry("mvsn_render_backward", false, scene, mlp_w, {rays_pts, rays_ndc, z_vals, rays_dir}, N, S,
+                          MVSN_MLP_FP32, false, nullptr, g, grad_mlp, grad_volume_dhwc, workspace, workspace_bytes, stream);
+}
+
+size_t mvsn_render_backward_tc_workspace_bytes(int N, int S) {
+    return backward_bytes(false, N, S, 0, 0, 0, MVSN_MLP_TC_HALF, false, false);
+}
+int mvsn_render_backward_tc(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                            const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                            const mvsn_render_grads* g, float* const* grad_mlp, float* grad_volume_dhwc, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward_tc");
+    return backward_entry("mvsn_render_backward_tc", false, scene, mlp_w, {rays_pts, rays_ndc, z_vals, rays_dir}, N, S,
+                          MVSN_MLP_TC_HALF, false, nullptr, g, grad_mlp, grad_volume_dhwc, workspace, workspace_bytes,
+                          stream);
+}
+
+size_t mvsn_render_backward_deterministic_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode) {
+    return backward_bytes(false, N, S, D, Hp, Wp, grad_mode, true, false);
+}
+int mvsn_render_backward_deterministic(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                                       const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                                       int grad_mode, const mvsn_render_grads* g, float* const* grad_mlp,
+                                       float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward_deterministic");
+    return backward_entry("mvsn_render_backward_deterministic", false, scene, mlp_w,
+                          {rays_pts, rays_ndc, z_vals, rays_dir}, N, S, grad_mode, true, nullptr, g, grad_mlp,
+                          grad_volume_dhwc, workspace, workspace_bytes, stream);
+}
+
+size_t mvsn_render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
+    return backward_bytes(false, N, S, D, Hp, Wp, grad_mode, deterministic != 0, true);
+}
+int mvsn_render_backward_stop(const mvsn_render_scene* scene, const float* const* mlp_w, const float* rays_pts,
+                              const float* rays_ndc, const float* z_vals, const float* rays_dir, int N, int S,
+                              int grad_mode, int deterministic, float t_stop, const mvsn_render_grads* g,
+                              float* const* grad_mlp, float* grad_volume_dhwc, int* live_samples,
+                              unsigned long long* tiles_done, void* workspace, size_t workspace_bytes, void* stream) {
+    MVSN_RANGE("mvsn_render_backward_stop");
+    const BwdStop stop{t_stop, live_samples, tiles_done};
+    return backward_entry("mvsn_render_backward_stop", false, scene, mlp_w, {rays_pts, rays_ndc, z_vals, rays_dir}, N, S,
+                          grad_mode, deterministic != 0, &stop, g, grad_mlp, grad_volume_dhwc, workspace,
+                          workspace_bytes, stream);
+}
+
+size_t mvsn_render_backward_rays_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
+    return backward_bytes(true, N, S, D, Hp, Wp, grad_mode, deterministic != 0, false);
+}
 int mvsn_render_backward_rays(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
                               const float* rays, const float* t_steps, const float* jitter, int N, int S, int grad_mode,
                               int deterministic, const mvsn_render_grads* g, float* const* grad_mlp,
                               float* grad_volume_dhwc, void* workspace, size_t workspace_bytes, void* stream) {
     MVSN_RANGE("mvsn_render_backward_rays");
-    return backward_rays_entry("mvsn_render_backward_rays", scene, mlp_w, rp, rays, t_steps, jitter, N, S, grad_mode,
-                               deterministic, g, grad_mlp, grad_volume_dhwc, workspace, workspace_bytes, stream, nullptr);
+    return backward_entry("mvsn_render_backward_rays", true, scene, mlp_w,
+                          {nullptr, nullptr, nullptr, nullptr, rp, rays, t_steps, jitter}, N, S, grad_mode,
+                          deterministic != 0, nullptr, g, grad_mlp, grad_volume_dhwc, workspace, workspace_bytes, stream);
 }
 
 size_t mvsn_render_backward_rays_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, int deterministic) {
-    if (!rays_grad_mode(grad_mode)) return 0;
-    return render_backward_stop_workspace_bytes(N, S, D, Hp, Wp, grad_mode, deterministic != 0);
+    return backward_bytes(true, N, S, D, Hp, Wp, grad_mode, deterministic != 0, true);
 }
-
 int mvsn_render_backward_rays_stop(const mvsn_render_scene* scene, const float* const* mlp_w, const mvsn_ray_params* rp,
                                    const float* rays, const float* t_steps, const float* jitter, int N, int S,
                                    int grad_mode, int deterministic, float t_stop, const mvsn_render_grads* g,
@@ -699,8 +649,9 @@ int mvsn_render_backward_rays_stop(const mvsn_render_scene* scene, const float* 
                                    unsigned long long* tiles_done, void* workspace, size_t workspace_bytes, void* stream) {
     MVSN_RANGE("mvsn_render_backward_rays_stop");
     const BwdStop stop{t_stop, live_samples, tiles_done};
-    return backward_rays_entry("mvsn_render_backward_rays_stop", scene, mlp_w, rp, rays, t_steps, jitter, N, S, grad_mode,
-                               deterministic, g, grad_mlp, grad_volume_dhwc, workspace, workspace_bytes, stream, &stop);
+    return backward_entry("mvsn_render_backward_rays_stop", true, scene, mlp_w,
+                          {nullptr, nullptr, nullptr, nullptr, rp, rays, t_steps, jitter}, N, S, grad_mode,
+                          deterministic != 0, &stop, g, grad_mlp, grad_volume_dhwc, workspace, workspace_bytes, stream);
 }
 
 int mvsn_adam_step(float* const* params, const float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,

@@ -1562,15 +1562,23 @@ static int bwd_grid(int N, int S) {
     return ngroups < sm_count() ? ngroups : sm_count();
 }
 
+// f(std::bool_constant<b0>{}, std::bool_constant<b1>{}, ...) for the runtime flags b0, b1, ...: the kernel variant
+// the flags select, with every combination instantiated once
+template <bool... B, class F>
+static int with_flags(F&& f) { return f(std::bool_constant<B>{}...); }
+template <bool... B, class F, class... Flags>
+static int with_flags(F&& f, bool b, Flags... rest) {
+    return b ? with_flags<B..., true>(f, rest...) : with_flags<B..., false>(f, rest...);
+}
+
 // One backward-kernel launch of the variant (grad_mode, DET, FAST, STOP); wh is the fp16 weight image (tensor-core
-// modes) or unused.  MVSN_GRAD_TC_FULL exists for FAST only (the launcher rejects it otherwise).
-template <bool DET, bool FAST, bool STOP = false>
+// modes) or unused.  MVSN_GRAD_TC_FULL exists for FAST only (the entries reject it otherwise).
+template <bool DET, bool FAST, bool STOP>
 static int launch_bwd_kernel(int grad_mode, int grid, const SceneDev& sc, const RenderIO& io, const BwdIO& bw,
                              const float* wts, const __half* wh, const DetIO& dt, const float* jitter, cudaStream_t stream,
-                             const StopIO& stop = StopIO{}) {
+                             const StopIO& stop) {
     static bool attr_set[3][64] = {};
     const int v = grad_mode == MVSN_GRAD_TC_FULL ? 2 : grad_mode == MVSN_MLP_TC_HALF ? 1 : 0;
-    MVSN_REQUIRE(FAST || v < 2, MVSN_EUNSUPPORTED, "MVSN_GRAD_TC_FULL: rays entries only");
     const void* kfn = (const void*)render_bwd_kernel<DET, FAST, STOP>;
     if (v == 1) kfn = (const void*)render_bwd_tc_kernel<DET, FAST, STOP>;
     if constexpr (FAST) { if (v == 2) kfn = (const void*)render_bwd_tc_kernel<DET, FAST, STOP, true>; }
@@ -1590,125 +1598,78 @@ static int launch_bwd_kernel(int grad_mode, int grid, const SceneDev& sc, const 
 
 }  // namespace
 
-size_t render_backward_workspace_bytes(int N, int S) {
-    if (S <= 0 || S > TILE_M || N <= 0) return 0;
-    const size_t ctas = (size_t)sm_count();              // sized for the widest launch on this device
-    return (ctas * (bwd::SCRATCH + bwd::GRADS) + bwd::DGRAD) * sizeof(float);
-}
-
-size_t render_backward_tc_workspace_bytes(int N, int S) {
-    if (S <= 0 || S > TILE_M || N <= 0) return 0;
-    const size_t ctas = (size_t)sm_count();
-    return ctas * (bwd::SCRATCH + bwd::GRADS) * sizeof(float) + bwdtc::WIMG * sizeof(__half);
-}
-
-// MVSN_GRAD_TC_FULL: the TC_HALF workspace with the forward's two extra weight operands in the fp16 image
-static size_t render_backward_tcf_workspace_bytes(int N, int S) {
-    if (S <= 0 || S > TILE_M || N <= 0) return 0;
-    const size_t ctas = (size_t)sm_count();
-    return ctas * (bwd::SCRATCH + bwd::GRADS) * sizeof(float) + bwdtc::WIMG_FULL * sizeof(__half);
-}
-
-// the workspace of a grad_mode's kernel (MVSN_MLP_FP32, MVSN_MLP_TC_HALF or MVSN_GRAD_TC_FULL)
-size_t render_backward_mode_workspace_bytes(int N, int S, int grad_mode) {
-    return grad_mode == MVSN_GRAD_TC_FULL ? render_backward_tcf_workspace_bytes(N, S)
-         : grad_mode == MVSN_MLP_TC_HALF  ? render_backward_tc_workspace_bytes(N, S)
-                                          : render_backward_workspace_bytes(N, S);
-}
-
-// Deterministic variant: the workspace of the grad mode, then (256-byte aligned) the [N] loss terms, and with a volume
-// gradient the two amax words (in a 256-byte slot), the int64 accumulator [D,Hp,Wp,8] right behind them (one memset
-// zeroes both) and the [N*S][8] record.
-namespace {
-struct DetLayout { size_t loss, amax, acc, rec, total; };
-DetLayout det_layout(size_t base, int N, int S, size_t nvox) {
-    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    DetLayout l{};
-    l.loss = up(base);
-    l.amax = up(l.loss + (size_t)N * sizeof(float));
-    l.acc = l.amax + 256;
-    l.rec = up(l.acc + nvox * 8 * sizeof(long long));
-    l.total = nvox ? l.rec + (size_t)N * S * 8 * sizeof(float) : l.amax;
-    return l;
-}
-}  // namespace
-
-size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode) {
+BwdLayout backward_layout(int N, int S, int D, int Hp, int Wp, int grad_mode, bool det, bool stop) {
+    BwdLayout l{};
     const bool frozen = D == 0 && Hp == 0 && Wp == 0;
-    if (!frozen && (D <= 0 || Hp <= 0 || Wp <= 0)) return 0;
-    const size_t base = render_backward_mode_workspace_bytes(N, S, grad_mode);
-    if (base == 0) return 0;
-    return det_layout(base, N, S, (size_t)D * Hp * Wp).total;
-}
-
-// Early ray termination: the workspace of the grad mode and summation order, then (256-byte aligned) the [N] live
-// counts and the CTAs' deferred-ray lists, list_cap (ray, live samples) pairs per CTA: every ray of its phase-A groups.
-namespace {
-struct StopLayout { size_t live, list, total; int list_cap; };
-StopLayout stop_layout(size_t base, int N, int S) {
+    if (S <= 0 || S > TILE_M || N <= 0 || (det && !frozen && (D <= 0 || Hp <= 0 || Wp <= 0))) return l;
+    // the dgrad weight image behind the per-CTA buffers: fp32, or fp16 for the tensor-core kernel (GRAD_TC_FULL: with
+    // the forward's two extra weight operands)
+    size_t wimg;
+    if (grad_mode == MVSN_MLP_FP32) wimg = bwd::DGRAD * sizeof(float);
+    else if (grad_mode == MVSN_MLP_TC_HALF) wimg = bwdtc::WIMG * sizeof(__half);
+    else if (grad_mode == MVSN_GRAD_TC_FULL) wimg = bwdtc::WIMG_FULL * sizeof(__half);
+    else return l;
     auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const int R = TILE_M / S, ngroups = (N + R - 1) / R, grid = bwd_grid(N, S);
-    StopLayout l{};
-    l.list_cap = (ngroups + grid - 1) / grid * R;
-    l.live = up(base);
-    l.list = up(l.live + (size_t)N * sizeof(int));
-    l.total = l.list + (size_t)grid * l.list_cap * sizeof(int2);
+    const size_t ctas = (size_t)sm_count();              // sized for the widest launch on this device
+    size_t end = ctas * (bwd::SCRATCH + bwd::GRADS) * sizeof(float) + wimg;
+    // deterministic: (256-byte aligned) the [N] loss terms, and with a volume gradient the two amax words (in a 256-byte
+    // slot), the int64 accumulator [D,Hp,Wp,8] right behind them (one memset zeroes both) and the [N*S][8] record
+    if (det) {
+        const size_t nvox = (size_t)D * Hp * Wp;
+        l.loss = up(end);
+        l.amax = up(l.loss + (size_t)N * sizeof(float));
+        l.acc = l.amax + 256;
+        l.rec = up(l.acc + nvox * 8 * sizeof(long long));
+        end = nvox ? l.rec + (size_t)N * S * 8 * sizeof(float) : l.amax;
+    }
+    // early ray termination: (256-byte aligned) the [N] live counts and the CTAs' deferred-ray lists, list_cap (ray, live
+    // samples) pairs per CTA: every ray of its phase-A groups
+    if (stop) {
+        const int R = TILE_M / S, ngroups = (N + R - 1) / R, grid = bwd_grid(N, S);
+        l.list_cap = (ngroups + grid - 1) / grid * R;
+        l.live = up(end);
+        l.list = up(l.live + (size_t)N * sizeof(int));
+        end = l.list + (size_t)grid * l.list_cap * sizeof(int2);
+    }
+    l.total = end;
     return l;
 }
-}  // namespace
 
-size_t render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, bool det) {
-    const size_t base = det ? render_backward_det_workspace_bytes(N, S, D, Hp, Wp, grad_mode)
-                            : render_backward_mode_workspace_bytes(N, S, grad_mode);
-    return base ? stop_layout(base, N, S).total : 0;
-}
-
-int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const float* const* mlp_w,
-                           const float* g_rgb, const float* target, float inv_count, const float* g_depth,
-                           const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
-                           float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream, int grad_mode, bool det, const float* jitter,
-                           const BwdStop* stop) {
-    const bool fast = io.rays != nullptr, tc = grad_mode != MVSN_MLP_FP32;
-    const char* what = stop ? (fast ? "mvsn_render_backward_rays_stop" : "mvsn_render_backward_stop")
-                     : fast ? "mvsn_render_backward_rays"
-                            : det ? (tc ? "deterministic render backward (grad_mode TC_HALF)" : "deterministic render backward")
-                                  : (tc ? "render backward (grad_mode TC_HALF)" : "render backward");
-    MVSN_REQUIRE(io.S <= TILE_M, MVSN_EUNSUPPORTED, "%s: N_samples=%d > 128 is not implemented", what, io.S);
-    MVSN_REQUIRE(fast || grad_mode != MVSN_GRAD_TC_FULL, MVSN_EUNSUPPORTED, "%s: MVSN_GRAD_TC_FULL is for the rays entries",
-                 what);
-    const size_t base = render_backward_mode_workspace_bytes(io.N, io.S, grad_mode);
-    const size_t nvox = dvol ? (size_t)sc.D * sc.Hp * sc.Wp : 0;
-    const DetLayout dl = det_layout(base, io.N, io.S, nvox);
-    const StopLayout sl = stop_layout(det ? dl.total : base, io.N, io.S);
-    const size_t need = stop ? sl.total : det ? dl.total : base;
-    MVSN_REQUIRE(workspace && workspace_bytes >= need, MVSN_EWORKSPACE, "%s: workspace %zu < %zu bytes", what, workspace_bytes, need);
-    MVSN_REQUIRE(aligned16(workspace), MVSN_EALIGN, "%s: workspace must be 16-byte aligned", what);
+int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const BwdCall& call,
+                           cudaStream_t stream) {
+    const bool fast = io.rays != nullptr, tc = call.grad_mode != MVSN_MLP_FP32, vol = call.dvol != nullptr;
+    const BwdLayout l = backward_layout(io.N, io.S, vol ? sc.D : 0, vol ? sc.Hp : 0, vol ? sc.Wp : 0, call.grad_mode,
+                                        call.det, call.stop != nullptr);
+    MVSN_REQUIRE(call.workspace && call.workspace_bytes >= l.total, MVSN_EWORKSPACE, "%s: workspace %zu < %zu bytes",
+                 call.what, call.workspace_bytes, l.total);
+    MVSN_REQUIRE(aligned16(call.workspace), MVSN_EALIGN, "%s: workspace must be 16-byte aligned", call.what);
+    char* w8 = static_cast<char*>(call.workspace);
     DetIO dt{};
-    if (det) {
-        char* w8 = static_cast<char*>(workspace);
-        dt.loss_terms = reinterpret_cast<float*>(w8 + dl.loss);
-        if (dvol) {
-            dt.amax = reinterpret_cast<unsigned*>(w8 + dl.amax);
-            dt.rec = reinterpret_cast<float*>(w8 + dl.rec);
+    if (call.det) {
+        dt.loss_terms = reinterpret_cast<float*>(w8 + l.loss);
+        if (vol) {
+            dt.amax = reinterpret_cast<unsigned*>(w8 + l.amax);
+            dt.rec = reinterpret_cast<float*>(w8 + l.rec);
             // the workspace is shared between modes and callers may hand it over uninitialised: zero every call
-            MVSN_CUDA_CHECK(cudaMemsetAsync(w8 + dl.amax, 0, dl.rec - dl.amax, stream));
+            MVSN_CUDA_CHECK(cudaMemsetAsync(w8 + l.amax, 0, l.rec - l.amax, stream));
         }
     }
     const int grid = bwd_grid(io.N, io.S);
-    float* ws = static_cast<float*>(workspace);
+    float* ws = static_cast<float*>(call.workspace);
     const size_t ctas = (size_t)sm_count();
+    const mvsn_render_grads& g = *call.g;
     BwdIO bw{};
-    bw.g_rgb = g_rgb; bw.target = target; bw.inv_count = inv_count; bw.g_depth = g_depth; bw.g_weights = g_weights;
-    bw.g_alpha = g_alpha; bw.g_feat = g_feat; bw.dvol = dvol; bw.rgb_out = rgb_out; bw.depth_out = depth_out; bw.loss = loss;
+    bw.g_rgb = g.rgb; bw.target = g.target_rgb; bw.inv_count = g.loss_scale; bw.g_depth = g.depth; bw.g_weights = g.weights;
+    bw.g_alpha = g.alpha; bw.g_feat = g.input_feat; bw.dvol = call.dvol; bw.rgb_out = g.rgb_out; bw.depth_out = g.depth_out;
+    bw.loss = g.loss_out;
     bw.scratch = ws; bw.grads = ws + ctas * bwd::SCRATCH;
     float* wimg = ws + ctas * (bwd::SCRATCH + bwd::GRADS);   // the dgrad weight image: fp32, or fp16 for the tc kernel
     MlpPtrsB wp;
-    for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) wp.p[i] = mlp_w[i];
+    for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) wp.p[i] = call.mlp_w[i];
     __half* wh = reinterpret_cast<__half*>(wimg);
     if (tc) {
         pack_dgrad_half_kernel<<<64, 256, 0, stream>>>(wp, wh);
-        if (grad_mode == MVSN_GRAD_TC_FULL) {
+        if (call.grad_mode == MVSN_GRAD_TC_FULL) {
             MVSN_CUDA_CHECK(cudaGetLastError());
             pack_fwd_half_kernel<<<32, 256, 0, stream>>>(wp, wh);
         }
@@ -1718,49 +1679,40 @@ int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* 
     }
     MVSN_CUDA_CHECK(cudaGetLastError());
     StopIO st{};
-    if (stop) {
-        char* w8 = static_cast<char*>(workspace);
-        st.t_stop = stop->t_stop;
-        st.live = stop->live_samples ? stop->live_samples : reinterpret_cast<int*>(w8 + sl.live);
-        st.list = reinterpret_cast<int2*>(w8 + sl.list);
-        st.list_cap = sl.list_cap;
-        st.tiles_done = stop->tiles_done;
+    if (call.stop) {
+        st.t_stop = call.stop->t_stop;
+        st.live = call.stop->live_samples ? call.stop->live_samples : reinterpret_cast<int*>(w8 + l.live);
+        st.list = reinterpret_cast<int2*>(w8 + l.list);
+        st.list_cap = l.list_cap;
+        st.tiles_done = call.stop->tiles_done;
     }
-    const int gm = grad_mode;
-    const int rc = stop ? (det ? (fast ? launch_bwd_kernel<true, true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st)
-                                       : launch_bwd_kernel<true, false, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream, st))
-                               : (fast ? launch_bwd_kernel<false, true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream, st)
-                                       : launch_bwd_kernel<false, false, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream, st)))
-                 : det ? (fast ? launch_bwd_kernel<true, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
-                               : launch_bwd_kernel<true, false>(gm, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream))
-                       : (fast ? launch_bwd_kernel<false, true>(gm, grid, sc, io, bw, wts_fp32, wh, dt, jitter, stream)
-                               : launch_bwd_kernel<false, false>(gm, grid, sc, io, bw, wts_fp32, wh, dt, nullptr, stream));
+    const int rc = with_flags([&](auto STOP, auto DET, auto FAST) {
+        return launch_bwd_kernel<DET, FAST, STOP>(call.grad_mode, grid, sc, io, bw, wts_fp32, wh, dt, call.jitter, stream, st);
+    }, call.stop != nullptr, call.det, fast);
     if (rc) return rc;
     GradOut go;
-    for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) go.p[i] = grad_mlp[i];
+    for (int i = 0; i < MVSN_N_MLP_TENSORS; ++i) go.p[i] = call.grad_mlp[i];
     mlp_grad_reduce_kernel<<<dim3(16, MVSN_N_MLP_TENSORS), 256, 0, stream>>>(bw.grads, grid, go);
     MVSN_CUDA_CHECK(cudaGetLastError());
-    if (det && dvol) {
+    if (call.det && vol) {
         const long long nsamp = (long long)io.N * io.S;
-        auto* acc = reinterpret_cast<unsigned long long*>(static_cast<char*>(workspace) + dl.acc);
+        auto* acc = reinterpret_cast<unsigned long long*>(w8 + l.acc);
         const int gs = cdiv(nsamp * 64, 256) < sm_count() * 16 ? cdiv(nsamp * 64, 256) : sm_count() * 16;
-        if (stop && fast) det_scatter_kernel<true, true><<<gs, 256, 0, stream>>>(sc, nullptr, dt.rec, dt.amax, nsamp, acc, dvol,
-                                                                                 io, jitter, st.live);
-        else if (stop) det_scatter_kernel<false, true><<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, dvol,
-                                                                              io, nullptr, st.live);
-        else if (fast) det_scatter_kernel<true><<<gs, 256, 0, stream>>>(sc, nullptr, dt.rec, dt.amax, nsamp, acc, dvol, io,
-                                                                       jitter, nullptr);
-        else      det_scatter_kernel<false><<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, dvol, io, nullptr,
-                                                                   nullptr);
+        // io.ndc is NULL for the rays entries, call.jitter and st.live for the entries without them
+        with_flags([&](auto STOP, auto FAST) {
+            det_scatter_kernel<FAST, STOP><<<gs, 256, 0, stream>>>(sc, io.ndc, dt.rec, dt.amax, nsamp, acc, call.dvol, io,
+                                                                   call.jitter, st.live);
+            return 0;
+        }, call.stop != nullptr, fast);
         MVSN_CUDA_CHECK(cudaGetLastError());
-        const long long n2 = (long long)nvox * 4;               // (int64 pair, float pair) per thread step
+        const long long n2 = (long long)sc.D * sc.Hp * sc.Wp * 4;   // (int64 pair, float pair) per thread step
         const int gc = cdiv(n2, 256) < sm_count() * 8 ? cdiv(n2, 256) : sm_count() * 8;
         det_convert_kernel<<<gc, 256, 0, stream>>>(reinterpret_cast<const longlong2*>(acc), dt.amax, nsamp,
-                                                   reinterpret_cast<float2*>(dvol), n2);
+                                                   reinterpret_cast<float2*>(call.dvol), n2);
         MVSN_CUDA_CHECK(cudaGetLastError());
     }
-    if (det && loss && target) {                                // the terms exist only with the fused loss
-        loss_reduce_kernel<<<1, 1024, 0, stream>>>(dt.loss_terms, io.N, loss);
+    if (call.det && g.loss_out && g.target_rgb) {               // the terms exist only with the fused loss
+        loss_reduce_kernel<<<1, 1024, 0, stream>>>(dt.loss_terms, io.N, g.loss_out);
         MVSN_CUDA_CHECK(cudaGetLastError());
     }
     return MVSN_OK;

@@ -107,19 +107,19 @@ int pack_mlp_wg(const float* const* w, bool split, void* packed, cudaStream_t st
 // det: the volume gradient and the loss summed in a fixed order (bit-reproducible); io.rays set: the samples are
 // marched in the kernel from io.rays / io.t_steps, stratified by `jitter` [N,S] (NULL: none), instead of read from
 // io.pts / io.ndc / io.z / io.dirs
-size_t render_backward_workspace_bytes(int N, int S);
-size_t render_backward_tc_workspace_bytes(int N, int S);
-size_t render_backward_mode_workspace_bytes(int N, int S, int grad_mode);
-size_t render_backward_det_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode);
-size_t render_backward_stop_workspace_bytes(int N, int S, int D, int Hp, int Wp, int grad_mode, bool det);
-// early ray termination of the rays backward (mvsn_render_backward_rays_stop); live_samples / tiles_done may be NULL
+// backward_layout: byte offsets in one call's workspace (the grad mode's, then `det`'s and `stop`'s buffers); D = Hp =
+// Wp = 0: a frozen volume.  total == 0: an unsupported shape or grad mode.
+struct BwdLayout { size_t loss, amax, acc, rec, live, list, total; int list_cap; };
+BwdLayout backward_layout(int N, int S, int D, int Hp, int Wp, int grad_mode, bool det, bool stop);
+// early ray termination (the _stop entries); live_samples / tiles_done may be NULL
 struct BwdStop { float t_stop; int* live_samples; unsigned long long* tiles_done; };
-int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const float* const* mlp_w,
-                           const float* g_rgb, const float* target, float inv_count, const float* g_depth,
-                           const float* g_weights, const float* g_alpha, const float* g_feat, float* const* grad_mlp,
-                           float* dvol, float* rgb_out, float* depth_out, float* loss, void* workspace,
-                           size_t workspace_bytes, cudaStream_t stream, int grad_mode, bool det,
-                           const float* jitter = nullptr, const BwdStop* stop = nullptr);
+// one backward call, every argument but the workspace checked by the entry `what`; dvol NULL: a frozen volume
+struct BwdCall {
+    const char* what; const mvsn_render_grads* g; const float* const* mlp_w; float* const* grad_mlp; float* dvol;
+    void* workspace; size_t workspace_bytes; int grad_mode; bool det; const float* jitter; const BwdStop* stop;
+};
+int launch_render_backward(const SceneDev& sc, const RenderIO& io, const float* wts_fp32, const BwdCall& call,
+                           cudaStream_t stream);
 int launch_adam_tensors(float* const* p, const float* const* g, float* const* m, float* const* v, const int* n, int count,
                         float lr, float beta1, float beta2, float eps, int step, cudaStream_t stream);
 int launch_adam_volume(float* p, float* g_dhwc, float* m, float* v, long long nvox, int planar, float lr, float beta1,
